@@ -3,15 +3,20 @@
 
 Workload (N=1): 3840x2160 NV12 -> 1920x1080 BGRA, method=lanczos (8-tap, 6-bit taps), bt709
 16-235, chroma-site mpeg2.  One "step" = one batch of FRAMES_PER_STEP distinct frames drawn from
-a ring whose working set (>= 1.3 GB) is far larger than the 126 MB L2, so no L2 flush is needed.
+a ring whose working set (>= 1.3 GB) is far larger than the 50 MB L2, so no L2 flush is needed.
 
   value      whole-job Mpix/s (input pixels), frames resident in HBM, kernel launches only
   e2e        same metric through the C-ABI host call (pinned host buffers, H2D + kernel + D2H
              inside the timed region)
   roofline   algorithmic bytes (20 736 000 B/frame, SURVEY §8d) / CUDA-event kernel time vs the
              measured HBM copy bandwidth in MEASURED_PEAKS.json
-  cpu_baseline  the reference's own converter (oracle/_ref, compiled from /root/reference
-             sources) — or the oracle port if that library is absent — on the host cores
+  cpu_baseline  the reference's own converter (oracle/_ref, compiled from the reference's
+             sources by oracle/Makefile) — or the oracle port if that library is absent — on the host cores
+
+--dump-outputs DIR writes what the timed path returned in its last timed step (BGRA bytes as float32):
+bgra_frame0.npy, the step's first output frame in full, and bgra_sample.npy, the step's other frames at a
+fixed seeded set of byte positions.  Inputs are generated from fixed seeds, so two builds run with the
+same arguments can be compared output for output.
 
 N>1: one process per GPU (torchrun), independent streams, no collective on the data path
 (SURVEY §8e): "scaling": "weak".  `--impl reference` times the reference CPU path instead.
@@ -45,7 +50,7 @@ def measured_peak():
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s, not measured)"
 
 
 class ClockSampler:
@@ -128,15 +133,6 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(self.samples)}
 
 
-def ncu_traffic(kernel, frames_per_launch):
-    """dram bytes per launch of the dominant kernel from the committed ncu --set full capture (profiles/)"""
-    try:
-        t = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))[kernel]
-        return (t["dram_bytes_read"] + t["dram_bytes_write"]) * frames_per_launch / t["frames_per_launch"]
-    except Exception:
-        return None
-
-
 def cpu_baseline(seconds=10.0, threads=None):
     """time the reference's CPU converter on frames of the same workload"""
     import numpy as np
@@ -205,6 +201,21 @@ def run_reference(args):
                              "sample": f"{args.steps} steps x {per_step} frames; {note}"},
             "e2e": {"value": val, "unit": "Mpix/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
     print(json.dumps(line), flush=True)
+
+
+DUMP_SAMPLE = 131_072     # byte positions per output frame after the first: 31 frames x 131 072 x 4 B = 16 MB
+
+
+def dump_outputs(path, outs):
+    """the last timed step's outputs as float32: the first frame in full (1080 x 1920 x 4, 33 MB) and the other frames at
+    DUMP_SAMPLE byte positions drawn from a fixed seed (the same positions in every frame and every run)"""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    np.save(os.path.join(path, "bgra_frame0.npy"), outs[0].cpu().numpy().reshape(OH, OW, 4).astype(np.float32))
+    idx = np.sort(np.random.default_rng(2024).choice(OW * OH * 4, DUMP_SAMPLE, replace=False))
+    sample = np.stack([o.cpu().numpy()[idx] for o in outs[1:]]).astype(np.float32)
+    np.save(os.path.join(path, "bgra_sample.npy"), sample)
+    np.save(os.path.join(path, "bgra_sample_positions.npy"), idx.astype(np.float64))
 
 
 def run_extras(steps):
@@ -309,6 +320,9 @@ def run_ours(args):
         torch.cuda.cudart().cudaProfilerStop()
     ms = e0.elapsed_time(e1)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        o = ((args.steps - 1) % (RING // FRAMES_PER_STEP)) * FRAMES_PER_STEP
+        dump_outputs(args.dump_outputs, ring_out[o:o + FRAMES_PER_STEP])
 
     # ---- sustained: the same launches back to back for >= 2 s (an issue-bound kernel follows the SM clock, and the
     # clock under a seconds-long load is not the burst clock)
@@ -367,7 +381,6 @@ def run_ours(args):
         achieved = args.steps * FRAMES_PER_STEP * ALG_BYTES_PER_FRAME / (ms * 1e-3) / 1e9   # per GPU
         e2e_val = e2e_steps * e2e_frames * world * IN_PIX_PER_FRAME / e2e_s / 1e6
         ceil_val = e2e_steps * e2e_frames * world * IN_PIX_PER_FRAME / probe_s / 1e6
-        traffic = ncu_traffic(kname, FRAMES_PER_STEP)
         line = {
             "metric": METRIC, "value": value, "unit": "Mpix/s",
             "frames_per_s": frames / (ms * 1e-3),
@@ -380,8 +393,6 @@ def run_ours(args):
                        "kernel_variant": int(pinfo.kernel_variant), "parallelism": f"streams{world}", "numa": numa},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
                          "frac": achieved / peak,
-                         "traffic": traffic,
-                         "traffic_source": "dram__bytes_read+write of the committed ncu --set full capture (profiles/traffic.json), not measured in this run",
                          "peak_source": peak_src, "kernel": kname,
                          "alg_bytes_per_launch": FRAMES_PER_STEP * ALG_BYTES_PER_FRAME,
                          "us_per_launch": ms * 1e3 / args.steps},
@@ -422,8 +433,12 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the C1 / C4 / C5 block of the line")
     ap.add_argument("--sustained-seconds", type=float, default=2.5)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as .npy files (float32) to DIR")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
+    if args.impl == "reference" and args.dump_outputs:
+        ap.error("--dump-outputs dumps the CUDA path's outputs; it is not available with --impl reference")
     if args.impl == "reference":
         run_reference(args)
     else:

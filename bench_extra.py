@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench_extra.py — secondary BASELINE configs on one B200 (kernel-resident numbers):
+"""bench_extra.py — secondary BASELINE configs on one GPU (kernel-resident numbers):
   C1  cudavideoconvertscale: 1080p NV12 -> 720p BGRA, bilinear (configs[0], the element default)
   C4  cudacompositor: 16 x 1080p RGBA pads -> 3840x2160 RGBA   (configs[3])
   C5  cudaaudioresample: 48k -> 44.1k F32, 256 channels          (configs[4], shortened buffer)

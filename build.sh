@@ -1,13 +1,16 @@
 #!/bin/bash
-# Builds libb200dsp.so (the product: CUDA kernels + C-ABI) in-tree for sm_100a.
-# nvcc cross-compiles without a GPU; the .so travels to the GPU box with the snapshot.
+# Builds libb200dsp.so (the product: CUDA kernels + C-ABI) in-tree for the H100 (sm_90a).
+# nvcc cross-compiles without a GPU.
 set -e
 cd "$(dirname "$0")"
 SRC=gstreamer_b200/csrc
 OUT=gstreamer_b200/libb200dsp.so
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
-FLAGS="-gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC,-O3,-Wall,-ffp-contract=off -Xptxas -v"
+ARCH="-gencode arch=compute_90a,code=sm_90a"
+FLAGS="$ARCH -lineinfo -O3 -std=c++17 -Xcompiler -fPIC,-O3,-Wall,-ffp-contract=off -Xptxas -v"
 mkdir -p build
+# objects compiled with other flags (another architecture) are stale whatever their time stamps say
+if [ "$(cat build/flags 2>/dev/null)" != "$FLAGS" ]; then rm -f build/*.o; echo "$FLAGS" > build/flags; fi
 OBJS=""
 for f in $SRC/*.cu $SRC/*.cpp; do
   o=build/$(basename "$f").o
@@ -17,5 +20,5 @@ for f in $SRC/*.cu $SRC/*.cpp; do
   fi
   OBJS="$OBJS $o"
 done
-$NVCC -gencode arch=compute_100a,code=sm_100a -shared -o $OUT $OBJS -cudart static
+$NVCC $ARCH -shared -o $OUT $OBJS -cudart static
 echo "built $OUT"

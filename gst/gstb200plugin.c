@@ -1,4 +1,4 @@
-/* gst/gstb200plugin.c — plugin entry of the B200-native raw-frame DSP elements.
+/* gst/gstb200plugin.c — plugin entry of the CUDA raw-frame DSP elements.
  *
  * Exports gst_plugin_b200_get_desc / gst_plugin_b200_register through GST_PLUGIN_DEFINE
  * (gstreamer/gst/gstplugin.h:274-307) and registers the three elements the way
@@ -23,5 +23,5 @@ plugin_init (GstPlugin * plugin)
 }
 
 GST_PLUGIN_DEFINE (GST_VERSION_MAJOR, GST_VERSION_MINOR, b200,
-    "B200-native colourspace/scale, compositor and audio resampler (libb200dsp)",
+    "CUDA colourspace/scale, compositor and audio resampler (libb200dsp)",
     plugin_init, VERSION, "LGPL", PACKAGE, "https://example.invalid/gst-b200")

@@ -319,8 +319,8 @@ gst_cuda_audio_resample_class_init (GstCudaAudioResampleClass * klass)
           GST_AUDIO_RESAMPLER_FILTER_INTERPOLATION_CUBIC, G_PARAM_READWRITE | G_PARAM_STATIC_STRINGS));
   gst_element_class_add_static_pad_template (element, &ars_sink);
   gst_element_class_add_static_pad_template (element, &ars_src);
-  gst_element_class_set_static_metadata (element, "B200 audio resampler", "Filter/Converter/Audio/Hardware",
-      "Bit-exact audioresample (F32, kaiser) polyphase FIR on sm_100a (libb200dsp)", "b200-gst-dsp");
+  gst_element_class_set_static_metadata (element, "CUDA audio resampler", "Filter/Converter/Audio/Hardware",
+      "Bit-exact audioresample (F32, kaiser) polyphase FIR on sm_90a (libb200dsp)", "b200-gst-dsp");
   trans->start = ars_start;
   trans->stop = ars_stop;
   trans->get_unit_size = ars_get_unit_size;
@@ -329,7 +329,7 @@ gst_cuda_audio_resample_class_init (GstCudaAudioResampleClass * klass)
   trans->set_caps = ars_set_caps;
   trans->transform = ars_transform;
   trans->sink_event = ars_sink_event;
-  GST_DEBUG_CATEGORY_INIT (cuda_ars_debug, "cudaaudioresample", 0, "B200 audio resampler");
+  GST_DEBUG_CATEGORY_INIT (cuda_ars_debug, "cudaaudioresample", 0, "CUDA audio resampler");
 }
 
 static void

@@ -343,12 +343,12 @@ gst_b200_cuda_compositor_class_init (GstB200CudaCompositorClass * klass)
           "GPU device to use", -1, G_MAXINT, 0, G_PARAM_READWRITE | GST_PARAM_MUTABLE_READY | G_PARAM_STATIC_STRINGS));
   gst_element_class_add_static_pad_template_with_gtype (element, &comp_src, GST_TYPE_AGGREGATOR_PAD);
   gst_element_class_add_static_pad_template_with_gtype (element, &comp_sink, gst_b200_compositor_pad_get_type ());
-  gst_element_class_set_static_metadata (element, "B200 compositor", "Filter/Editor/Video/Compositor/Hardware",
-      "Bit-exact compositor alpha blend in one pass on sm_100a (libb200dsp)", "b200-gst-dsp");
+  gst_element_class_set_static_metadata (element, "CUDA compositor", "Filter/Editor/Video/Compositor/Hardware",
+      "Bit-exact compositor alpha blend in one pass on sm_90a (libb200dsp)", "b200-gst-dsp");
   agg->start = comp_start;
   agg->stop = comp_stop;
   vagg->aggregate_frames = comp_aggregate_frames;
-  GST_DEBUG_CATEGORY_INIT (cuda_comp_debug, "cudacompositor", 0, "B200 compositor");
+  GST_DEBUG_CATEGORY_INIT (cuda_comp_debug, "cudacompositor", 0, "CUDA compositor");
 }
 
 static void

@@ -546,9 +546,9 @@ gst_cuda_video_convert_scale_class_init (GstCudaVideoConvertScaleClass * klass)
 
   gst_element_class_add_static_pad_template (element, &sink_tmpl);
   gst_element_class_add_static_pad_template (element, &src_tmpl);
-  gst_element_class_set_static_metadata (element, "B200 colourspace converter and scaler",
+  gst_element_class_set_static_metadata (element, "CUDA colourspace converter and scaler",
       "Filter/Converter/Video/Scaler/Colorspace/Hardware",
-      "Bit-exact videoconvertscale on sm_100a (libb200dsp)", "b200-gst-dsp");
+      "Bit-exact videoconvertscale on sm_90a (libb200dsp)", "b200-gst-dsp");
   element->set_context = vcs_set_context;
 
   trans->passthrough_on_same_caps = TRUE;
@@ -561,7 +561,7 @@ gst_cuda_video_convert_scale_class_init (GstCudaVideoConvertScaleClass * klass)
   trans->transform = vcs_transform;
   trans->propose_allocation = vcs_propose_allocation;
   trans->decide_allocation = vcs_decide_allocation;
-  GST_DEBUG_CATEGORY_INIT (cuda_vcs_debug, "cudavideoconvertscale", 0, "B200 convert + scale");
+  GST_DEBUG_CATEGORY_INIT (cuda_vcs_debug, "cudavideoconvertscale", 0, "CUDA convert + scale");
 }
 
 static void

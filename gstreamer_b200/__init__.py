@@ -1,7 +1,7 @@
-"""gstreamer_b200 — B200-native raw-frame DSP hot path behind GStreamer's element surface.
+"""gstreamer_b200 — CUDA-native (H100, sm_90a) raw-frame DSP hot path behind GStreamer's element surface.
 
 Python is the test/bench harness and the host-side mirror of the reference's element
-interface; the product is gstreamer_b200/libb200dsp.so (hand-written sm_100a CUDA +
+interface; the product is gstreamer_b200/libb200dsp.so (hand-written sm_90a CUDA +
 C-ABI, include/b200dsp.h).  Importing this package without the built library fails.
 """
 from ._lib import lib, LIB_PATH, B200Error, EXPORTED_SYMBOLS, MISSING_SYMBOLS  # noqa: F401

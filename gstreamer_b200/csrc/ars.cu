@@ -1,4 +1,4 @@
-// gstreamer_b200/csrc/ars.cu — b200_ars_* : polyphase FIR audio resampler (product code, sm_100a).
+// gstreamer_b200/csrc/ars.cu — b200_ars_* : polyphase FIR audio resampler (product code, sm_90a).
 //
 // Replaces, for F32 interleaved audio with the audioresample element's defaults
 // (kaiser, filter-mode auto, cubic filter interpolation; gst/audioresample/gstaudioresample.c:68-72):
@@ -662,8 +662,8 @@ __device__ __forceinline__ long long sat_s32 (long long v) { return v < -2147483
 // integers (wrapping 32 bit like the SSE2 pmaddwd path), so no lane structure has to be kept —
 // inner_product_gint16_full_1_sse2 (audio-resampler-x86-sse2.c:29-56): sum, + 2^14, >> 15, saturate.
 // ---- ars_pipe_kernel: the tile kernel as a persistent, double-buffered pipeline ------------------------------------------
-// Profile of ars_tile_kernel on the C5 shape (profiles/r02_ars_*): 57 % of the stall samples sit in the prologue (window and
-// tap rows travelling from L2 to shared memory) although it is 16 % of the instructions - two CTAs per SM cannot hide it.
+// In ars_tile_kernel on the C5 shape the prologue (window and tap rows travelling from L2 to shared memory) stalls far more
+// than its share of the instructions - two CTAs per SM cannot hide it.
 // Here one CTA per SM (16 warps) walks its tiles (64 outputs x 128 channels) with TWO staging buffers: while the warps
 // multiply tile k, cp.async fills the window and the tap rows of tile k+1 (zero fill for silence / missing frames through
 // the src-size operand).  With registers no longer shared between CTAs a thread owns 4 adjacent channels x 4 outputs:
@@ -802,9 +802,8 @@ ars_pipe_kernel_v1 (const ArsLaunch L, const ArsTile Tl, int n_fb, int n_cb)
 }
 
 // ---- ars_pipe_kernel (second form): bulk copies + mbarriers, no CTA-wide barrier in the steady state ----------------------
-// Profile of the cp.async form above (profiles/r02_ars_pipe_ncu.txt): 3580 instructions per thread and tile of which 2560
-// are the FIR; ~280 were cp.async issue + its address arithmetic (4800 16-byte copies per tile), the two __syncthreads per
-// tile cost 0.47 stalled warps per issue, and the stage pointers selected from a two-entry array made the inner loop's
+// In the cp.async form above a tenth of the instructions are cp.async issue + its address arithmetic (4800 16-byte copies
+// per tile), the two __syncthreads per tile stall warps, and the stage pointers selected from a two-entry array made the inner loop's
 // loads generic (LD.E.128) instead of LDS.128.  Here a window row (CB channels of one frame, 512 contiguous bytes) and a
 // tap row (one 4-output group, nch * 64 bytes) each travel as ONE cp.async.bulk issued by one lane (166 per tile instead
 // of 6080 cp.async), completion is counted by an mbarrier per stage (full[2]), and the stage is handed back through a
@@ -952,7 +951,7 @@ ars_pipe_kernel (const ArsLaunch L, const ArsTile Tl, int n_fb, int n_cb, const 
     // a window that lies in the caller's input (every tile but the first few) is ONE tensor copy: box = CB channels x win
     // frames, rows past the end of the input arrive as zeros (out-of-bounds fill) like the missing frames of the row path.
     // (Divergent lanes issuing a bulk copy each are serialised through the uniform datapath: the row path below costs the
-    // producing warps ~40 copies each and made them the tile's stragglers - measured 1.77 ms against 1.72 for cp.async.)
+    // producing warps ~40 copies each and makes them the tile's stragglers.)
     const bool tensor = use_tm && f0 >= L.hist_frames;
     if (tensor) {
       if (warp == 0 && lane == 0) {
@@ -1117,7 +1116,7 @@ ars_pipe_kernel_s16 (const ArsLaunch L, const ArsTile Tl, int n_fb, int n_cb, co
     // a window that lies in the caller's input (every tile but the first few) is ONE tensor copy: box = CB channels x win
     // frames, rows past the end of the input arrive as zeros (out-of-bounds fill) like the missing frames of the row path.
     // (Divergent lanes issuing a bulk copy each are serialised through the uniform datapath: the row path below costs the
-    // producing warps ~40 copies each and made them the tile's stragglers - measured 1.77 ms against 1.72 for cp.async.)
+    // producing warps ~40 copies each and makes them the tile's stragglers.)
     const bool tensor = use_tm && f0 >= L.hist_frames;
     if (tensor) {
       if (warp == 0 && lane == 0) {
@@ -2057,7 +2056,7 @@ int b200_ars_process (b200_ars * h, const void *in_v, size_t in_frames, void *ou
     ArsTile tl = ArsTile ();
     int cb = 32 * (L.wcn > 4 ? 4 : L.wcn);
     { const char *e = getenv ("B200_ARS_CB"); if (e && (atoi (e) == 64 || atoi (e) == 32) && atoi (e) < cb) cb = atoi (e); }   // tuning knob
-    // channels per thread: 2 measured best on B200 (C5: 2.01 ms vs 2.44 ms for 1 and 2.57 ms for 4)
+    // channels per thread: 2 (B200_ARS_CPT overrides)
     int cpt = cb >= 64 ? 2 : 1;
     if (env_cpt && (atoi (env_cpt) == 1 || (atoi (env_cpt) == 4 && cb >= 128))) cpt = atoi (env_cpt);
     {

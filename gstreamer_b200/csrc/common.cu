@@ -30,11 +30,11 @@ int cuda_fail (cudaError_t e, const char *what, const char *file, int line)
 int sm_count (int device)
 {
   static int cache[64];
-  if (device < 0 || device >= 64) return 148;
+  if (device < 0 || device >= 64) return 132;
   if (cache[device] == 0) {
     int n = 0;
     if (cudaDeviceGetAttribute (&n, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || n <= 0)
-      n = 148;
+      n = 132;                                      // H100 SXM
     cache[device] = n;
   }
   return cache[device];
@@ -92,8 +92,8 @@ std::map<void *, size_t> g_registered;      // mmap'ed + cudaHostRegister'ed blo
 }
 
 // Staging memory on the NUMA node the device hangs off: with one pipeline per GPU on a two-socket host, page-locked
-// buffers that happen to sit on the other socket push every H2D / D2H byte across the socket interconnect (round 1:
-// per-GPU H2D fell from 49 to 22 GB/s at 8 pipelines).  Pages are bound with mbind(MPOL_BIND) BEFORE they are touched,
+// buffers that happen to sit on the other socket push every H2D / D2H byte across the socket interconnect.
+// Pages are bound with mbind(MPOL_BIND) BEFORE they are touched,
 // then locked and mapped with cudaHostRegister - the placement does not depend on which core the caller runs on.
 int b200_host_alloc_near (int device, size_t size, void **ptr)
 {

@@ -33,7 +33,7 @@ struct DeviceGuard {
 
 // Opt a kernel in to the device's full dynamic shared memory.  The attribute is per FUNCTION (and per device), not per
 // handle: plans of different footprints share the kernels, so the limit is always raised to the device's opt-in maximum
-// (227 KB on sm_100) and never to one plan's own size — a later, smaller handle must not lower it under an earlier one.
+// (227 KB on sm_90) and never to one plan's own size — a later, smaller handle must not lower it under an earlier one.
 // The limit itself costs nothing; occupancy follows the bytes each launch actually asks for.
 template <typename F>
 int allow_max_dyn_smem (F fn)

@@ -1,4 +1,4 @@
-// gstreamer_b200/csrc/comp.cu — b200_comp_* : single-pass compositor (product code, sm_100a).
+// gstreamer_b200/csrc/comp.cu — b200_comp_* : single-pass compositor (product code, sm_90a).
 //
 // Replaces the per-pad read-modify-write passes of the reference
 //   blend_pads()/_draw_background()      gst-plugins-base/gst/compositor/compositor.c:1619-1697
@@ -212,8 +212,8 @@ comp_kernel (const CompParams P)
 #pragma unroll
     for (int i = 0; i < 4; i++) d[i] = i < n ? dp[i] : 0u;
   }
-  // (fetching the next covering pad's pixels while the current one is blended was measured and dropped: 56.7 against 48.5 us
-  //  per C4 frame - 40 registers instead of 32 cost more occupancy than the overlap returned, profiles/r02_comp_prefetch.txt)
+  // (fetching the next covering pad's pixels while the current one is blended was tried and dropped:
+  //  40 registers instead of 32 cost more occupancy than the overlap returned)
   for (int k = 0; k < count; k++) {
     const CompTilePad & p = s_pads[k];
     const int full = p.full;

@@ -12,7 +12,7 @@
 #include "vcs_lanczos2_v2.cuh"
 #include "vcs_l2mma.cuh"
 #ifndef B200_CUDA_EMU
-#include "vcs_l2tc.cuh"          // tcgen05 / TMEM: no host emulation
+#include "vcs_l2tc.cuh"          // wgmma: no host emulation
 #endif
 #include "vcs_light.cuh"
 #include "vcs_ntap.cuh"
@@ -51,7 +51,7 @@ struct b200_vcs {
   L2mmaTables mma_tables;         // experimental tensor-path variant of the 2:1 kernel (variant 6, opt-in)
   L2mmaState mma;
 #ifndef B200_CUDA_EMU
-  L2tcTables tc_tables;           // tcgen05 formulation of the 2:1 kernel (variant 7)
+  L2tcTables tc_tables;           // tensor-core (wgmma) formulation of the 2:1 kernel (variant 7)
   L2tcState tc;
 #endif
   PlanesState planes;
@@ -631,8 +631,8 @@ int b200_vcs_create (const b200_video_info * in, const b200_video_info * out,
       h->variant = 3;
     }
   }
-  // variant 6 (mma.sync formulation of the 2:1 kernel) measured 12.7 us/frame against 8.4 for the SIMT kernel
-  // (profiles/r02_first_bench_l2mma.json): kept selectable through b200_vcs_set_kernel_variant for cross-checks only
+  // variant 6 (mma.sync formulation of the 2:1 kernel) is not timed on the H100 and not the default: kept selectable
+  // through b200_vcs_set_kernel_variant for cross-checks only
   *handle = h;
   return B200_OK;
 }
@@ -698,7 +698,7 @@ int b200_vcs_convert_host (b200_vcs * h, int n, const void *const *in_host, void
   // of chunk c-1 overlap the kernel of chunk c (the copy engines run beside the SMs).  One kernel launch and one event
   // triple per chunk, not per frame; with few frames the chunk shrinks so that all three stages still overlap.
   const int K = b200_vcs::kSlots;
-  // measured: 16 frames in chunks of 4 lose 14 % to pipeline fill / drain against single frames
+  // chunks only for long calls: with few frames per call the pipeline's fill and drain would outweigh what chunking saves
   const int chunk = n >= 16 * b200_vcs::kChunk ? b200_vcs::kChunk : (n >= 32 ? 2 : 1);
   int st = ensure_pipeline (h, chunk);
   if (st != B200_OK) return st;

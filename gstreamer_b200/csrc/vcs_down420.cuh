@@ -1,4 +1,4 @@
-// gstreamer_b200/csrc/vcs_down420.cuh — chroma down-sampling + 4:2:0 pack (product, sm_100a).
+// gstreamer_b200/csrc/vcs_down420.cuh — chroma down-sampling + 4:2:0 pack (product, sm_90a).
 //
 // Second launch of the 4:2:0 -> other-4:2:0-family path (NV12 <-> I420, NV12 <-> NV21 ...), which the reference runs
 // through its generic chain: after the scalers, chain_downsample (video-converter.c:2018-2032, do_downsample_lines

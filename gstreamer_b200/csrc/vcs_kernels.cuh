@@ -1,4 +1,4 @@
-// gstreamer_b200/csrc/vcs_kernels.cuh — convert+scale device code (product, sm_100a).
+// gstreamer_b200/csrc/vcs_kernels.cuh — convert+scale device code (product, sm_90a).
 //
 // Integer arithmetic here reproduces, stage by stage, what the reference's ORC
 // programs compute (gst-libs/gst/video/video-orc.orc); each helper cites its program.

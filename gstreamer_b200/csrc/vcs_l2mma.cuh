@@ -1,12 +1,12 @@
-// gstreamer_b200/csrc/vcs_l2mma.cuh — experimental variant of the headline kernel (product code, sm_100a; opt-in).
+// gstreamer_b200/csrc/vcs_l2mma.cuh — experimental variant of the headline kernel (product code, sm_90a; opt-in).
 //
 // Same shape class and the same arithmetic as vcs_lanczos2_kernel (4:2:0 semi-planar -> packed RGB, exact 2:1 in both
 // directions, 8-tap filters, h-cosited chroma, lines consumed in order), but the two FIR passes run on the integer
 // tensor path: a 2:1 8-tap FIR over u8 samples with s8 taps and exact s32 accumulation IS a banded matrix product, and
 // IMMA.16832.U8.S8 (mma.sync.m16n8k32) computes 128 FIR outputs per warp instruction where the SIMT kernel spends
 // 2-3 IDP.4A plus alignment work per output.  The measured limiter of the SIMT kernel is instruction issue
-// (DESIGN.md 4.2), which is what this variant attacks; whether it wins is a measurement for the next device session —
-// until then it is selected only by B200_L2_MMA=1 or b200_vcs_set_kernel_variant (h, 6).
+// (DESIGN.md 4.2), which is what this variant attacks; it has not been timed on the H100 and is
+// selected only by b200_vcs_set_kernel_variant (h, 6).
 //
 //  stage A  a thread prepares 4 lines x 8 input pixels: Y copied, chroma de-interleaved, co-sited h up-sampling and the
 //           (3a+b+2)>>2 line pairs as packed byte averages (the code of vcs_lanczos2_kernel's H phase), written as planar

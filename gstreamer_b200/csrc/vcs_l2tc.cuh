@@ -1,22 +1,20 @@
-// gstreamer_b200/csrc/vcs_l2tc.cuh — the exact-2:1 / 8-tap kernel with both FIR passes on the 5th-generation tensor
-// cores (product code, sm_100a only: tcgen05.mma.kind::i8 with TMEM accumulators).
+// gstreamer_b200/csrc/vcs_l2tc.cuh — the exact-2:1 / 8-tap kernel with both FIR passes on the Hopper tensor cores
+// (product code, sm_90a: wgmma.mma_async with s8 x u8 operands from shared memory and s32 accumulators in registers).
 //
-// Why: the measured ablation of vcs_lanczos2_kernel (profiles/r02_l2_ablation_*.txt) puts 1.15 us/frame in the horizontal
-// FIR's dot products alone and as much again in the shuffles, shifts and packs around it, against an HBM floor of 3.2 us:
-// the SIMT kernel is bound by integer issue, not by memory.  Both FIRs are banded u8 x s8 matrix products with exact
-// 32-bit accumulation, so they can leave the issue slots altogether:
+// Why: the SIMT 2:1 kernel spends most of its issue slots on the horizontal FIR's dot products and the shuffles, shifts
+// and packs around them.  Both FIRs are banded u8 x s8 matrix products with exact 32-bit accumulation, so they can run
+// on the tensor cores instead:
 //
 //   H pass   D_h[j][l] = sum_x band[j][x] * img[l][x]       A = tap band of the strip's 128 output columns (s8, K-major)
 //                                                           B = the staged input lines of one channel (u8, K = pixels)
 //   V pass   D_v[c][r] = sum_l hs[c][l]   * vband[r][l]     A = h-scaled samples, one row per output column (u8, K = lines)
 //                                                           B = tap band of the tile's output rows (s8)
 //
-// With the band as the A operand the accumulator of an output COLUMN lives in one TMEM lane, so the thread that owns the
-// lane reads consecutive LINES of its column, packs four of them per word and writes the V pass's K-major operand with
-// 16-byte stores; the V accumulators come back one output column per lane again, which makes the final stores coalesced
-// rows.  Rounding is one more K step against a block of ones ((acc + 32) >> 6, or taps times 4 and + 128 so that the
-// saturated result is byte 1 of a 16-bit saturating pack); garbage in staged samples outside the frame meets zero taps
-// (the reference folds its edge taps inward, see pack of the bands below), so no clamped copies are needed.
+// Each of the two warpgroups owns 64 of the strip's 128 output columns (wgmma M = 64) in both passes, so the h-scaled
+// operand a warpgroup writes after its H pass is read only by its own V pass.  Rounding is one more K step against a
+// block of ones ((acc + 32) >> 6, or taps times 4 and + 128 so that the saturated result is byte 1 of a 16-bit
+// saturating pack); garbage in staged samples outside the frame meets zero taps (the reference folds its edge taps
+// inward, see pack of the bands below), so no clamped copies are needed.
 // What stays SIMT is what is not linear: de-interleaving and the two rounding chroma up-sampling steps
 // (video-chroma.c:687-699, video-orc.orc:2705-2735), saturation, and the AYUV -> ARGB mulhi matrix.
 //
@@ -36,10 +34,11 @@
 
 namespace b200 {
 
-constexpr int TC_THREADS = 256;
-constexpr int TC_TW = 128;                                 // output columns per tile = rows of the band (UMMA M)
+constexpr int TC_THREADS = 256;                            // two warpgroups
+constexpr int TC_PROD_WARPS = TC_THREADS / 32;             // every warp stages
+constexpr int TC_TW = 128;                                 // output columns per tile = rows of the band (2 x wgmma M)
 constexpr int TC_TH = 28;                                  // output rows per tile
-constexpr int TC_N = 64;                                   // staged input lines (2 * TH + 6 = 62 used) = UMMA N of the H pass
+constexpr int TC_N = 64;                                   // staged input lines (2 * TH + 6 = 62 used) = wgmma N of the H pass
 constexpr int TC_CHUNKS = 18;                              // 16-byte chunks per staged line: 288 input bytes (2 * 128 + 6, 16-aligned start)
 constexpr int TC_X_LEAD = 16;                              // the staged window starts 16 pixels left of the strip's first tap centre - 3
 constexpr int TC_IMG_LBO = 8 * 128 + 16;                   // bytes between chunk columns of a staged plane (+16: bank spread)
@@ -48,7 +47,7 @@ constexpr int TC_BAND_CHUNKS = TC_CHUNKS + 2;              // + the rounding K s
 constexpr int TC_BAND_LBO = 16 * 128;                      // 128 rows
 constexpr int TC_BAND_BYTES = TC_BAND_CHUNKS * TC_BAND_LBO;   // 40 960
 constexpr int TC_ONES_BYTES = 2 * TC_BAND_LBO;             // [2 chunks][128 rows][16]: every byte 1
-constexpr int TC_VROWS = 32;                               // UMMA N of the V pass (28 used)
+constexpr int TC_VROWS = 32;                               // wgmma N of the V pass (28 used)
 constexpr int TC_VB_CHUNKS = TC_N / 16 + 2;
 constexpr int TC_VB_LBO = (TC_VROWS / 8) * 128;            // 512
 constexpr int TC_VB_BYTES = TC_VB_CHUNKS * TC_VB_LBO;      // 3 072
@@ -58,12 +57,11 @@ constexpr int TC_HS_BYTES = (TC_N / 16) * TC_HS_LBO;       // per channel 8 192
 constexpr int TC_OFF_BAND = 0;
 constexpr int TC_OFF_ONES = TC_OFF_BAND + TC_BAND_BYTES;
 constexpr int TC_OFF_VB = TC_OFF_ONES + TC_ONES_BYTES;
-constexpr int TC_OFF_IMG = TC_OFF_VB + TC_VB_BYTES;         // 3 planes; the h-scaled operand re-uses this space after the H pass
-constexpr int TC_OFF_BAR = TC_OFF_IMG + 3 * TC_IMG_BYTES;
-constexpr int TC_SMEM = TC_OFF_BAR + 64;
-constexpr int TC_TMEM_COLS = 256;                           // 3 x 64 accumulator columns (H), re-used as 3 x 32 (V)
-static_assert (3 * TC_HS_BYTES <= 3 * TC_IMG_BYTES, "h-scaled operand must fit the staged planes");
-static_assert (TC_OFF_IMG % 16 == 0 && TC_IMG_BYTES % 16 == 0, "operand alignment");
+constexpr int TC_OFF_IMG = TC_OFF_VB + TC_VB_BYTES;         // 3 planes
+constexpr int TC_OFF_HS = TC_OFF_IMG + 3 * TC_IMG_BYTES;    // 3 channels of the V pass's A operand
+constexpr int TC_SMEM = TC_OFF_HS + 3 * TC_HS_BYTES;        // 128 864: one CTA per SM
+static_assert (TC_OFF_IMG % 16 == 0 && TC_IMG_BYTES % 16 == 0 && TC_OFF_HS % 16 == 0, "operand alignment");
+static_assert (TC_SMEM <= 227 * 1024, "one CTA must fit the opt-in shared memory of sm_90");
 
 struct L2tcDev {
   const uint8_t *band;          // [strips][TC_BAND_BYTES]   tap band of each 128-column strip, canonical layout, + rounding step
@@ -73,56 +71,17 @@ struct L2tcDev {
   unsigned magic_rt;            // 2^32 / row_tiles + 1: t / row_tiles == umulhi (t, magic) for the tile counts that occur
 };
 
-// ---- PTX wrappers (sm_100a) -----------------------------------------------------------------------------------------
+// ---- PTX wrappers (sm_90a) ------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t tc_smem_u32 (const void *p) { return (uint32_t) __cvta_generic_to_shared (p); }
 __device__ __forceinline__ uint64_t tc_desc (uint32_t saddr, uint32_t lbo, uint32_t sbo)
 {
-  // matrix descriptor, un-swizzled K-major: start >> 4 | LBO >> 4 << 16 | SBO >> 4 << 32 | version 1 << 46 | layout 0 << 61
+  // wgmma matrix descriptor, no swizzle (layout 0 at bits 62-63): start >> 4 | LBO >> 4 << 16 | SBO >> 4 << 32
   return (uint64_t) ((saddr >> 4) & 0x3fffu) | ((uint64_t) ((lbo >> 4) & 0x3fffu) << 16) |
-      ((uint64_t) ((sbo >> 4) & 0x3fffu) << 32) | ((uint64_t) 1 << 46);
-}
-// instruction descriptor for kind::i8: D = s32, A / B formats (0 = u8, 1 = s8), both K-major, N >> 3 at bit 17, M >> 4 at bit 24
-__host__ __device__ constexpr uint32_t tc_idesc (int a_signed, int b_signed, int n, int m)
-{
-  return (2u << 4) | ((uint32_t) a_signed << 7) | ((uint32_t) b_signed << 10) | ((uint32_t) (n >> 3) << 17) | ((uint32_t) (m >> 4) << 24);
-}
-__device__ __forceinline__ void tc_mma (uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-#ifndef B200_CUDA_EMU
-  asm volatile ("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, {%5, %5, %5, %5}, p;\n\t}\n"
-      :: "r" (d_tmem), "l" (adesc), "l" (bdesc), "r" (idesc), "r" (accumulate), "r" (0u) : "memory");
-#endif
-}
-__device__ __forceinline__ void tc_commit (uint32_t bar)
-{
-#ifndef B200_CUDA_EMU
-  asm volatile ("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r" (bar) : "memory");
-#endif
-}
-__device__ __forceinline__ void tc_fence_before () {
-#ifndef B200_CUDA_EMU
-  asm volatile ("tcgen05.fence::before_thread_sync;" ::: "memory");
-#endif
-}
-__device__ __forceinline__ void tc_fence_after () {
-#ifndef B200_CUDA_EMU
-  asm volatile ("tcgen05.fence::after_thread_sync;" ::: "memory");
-#endif
+      ((uint64_t) ((sbo >> 4) & 0x3fffu) << 32);
 }
 __device__ __forceinline__ void tc_fence_async_smem () {
 #ifndef B200_CUDA_EMU
   asm volatile ("fence.proxy.async.shared::cta;" ::: "memory");
-#endif
-}
-__device__ __forceinline__ void tc_bar_wait (uint32_t bar, uint32_t parity)
-{
-#ifndef B200_CUDA_EMU
-  uint32_t ok;
-  do {
-    asm volatile ("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-        : "=r" (ok) : "r" (bar), "r" (parity) : "memory");
-  } while (!ok);
 #endif
 }
 __device__ __forceinline__ void tc_cp16 (uint32_t saddr, const void *g)
@@ -137,133 +96,100 @@ __device__ __forceinline__ void tc_cp_wait ()
   asm volatile ("cp.async.wait_all;" ::: "memory");
 #endif
 }
-#define TC_LD16(v, taddr)                                                                                          \
-  asm volatile ("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"  \
-      : "=r" (v[0]), "=r" (v[1]), "=r" (v[2]), "=r" (v[3]), "=r" (v[4]), "=r" (v[5]), "=r" (v[6]), "=r" (v[7]),       \
-        "=r" (v[8]), "=r" (v[9]), "=r" (v[10]), "=r" (v[11]), "=r" (v[12]), "=r" (v[13]), "=r" (v[14]), "=r" (v[15])   \
-      : "r" (taddr) : "memory")
-__device__ __forceinline__ void tc_ld_wait () {
+__device__ __forceinline__ void tc_wg_fence () {
 #ifndef B200_CUDA_EMU
-  asm volatile ("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+  asm volatile ("wgmma.fence.sync.aligned;" ::: "memory");
+#endif
+}
+__device__ __forceinline__ void tc_wg_commit_wait () {
+#ifndef B200_CUDA_EMU
+  asm volatile ("wgmma.commit_group.sync.aligned;" ::: "memory");
+  asm volatile ("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+#endif
+}
+// the accumulators are written asynchronously: no use of them may be scheduled before the wait
+template <int N>
+__device__ __forceinline__ void tc_fence_regs (int (&d)[N])
+{
+#pragma unroll
+  for (int i = 0; i < N; i++) asm volatile ("" : "+r" (d[i]) :: "memory");
+}
+
+// H pass step: D (64 columns x 64 lines, s32) (+)= band (s8) x img (u8)
+__device__ __forceinline__ void tc_mma_h (int (&d)[32], uint64_t adesc, uint64_t bdesc, int accumulate)
+{
+#ifndef B200_CUDA_EMU
+  asm volatile ("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.u8 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31},"
+      " %32, %33, p;\n\t}\n"
+      : "+r" (d[0]), "+r" (d[1]), "+r" (d[2]), "+r" (d[3]), "+r" (d[4]), "+r" (d[5]), "+r" (d[6]), "+r" (d[7]),
+        "+r" (d[8]), "+r" (d[9]), "+r" (d[10]), "+r" (d[11]), "+r" (d[12]), "+r" (d[13]), "+r" (d[14]), "+r" (d[15]),
+        "+r" (d[16]), "+r" (d[17]), "+r" (d[18]), "+r" (d[19]), "+r" (d[20]), "+r" (d[21]), "+r" (d[22]), "+r" (d[23]),
+        "+r" (d[24]), "+r" (d[25]), "+r" (d[26]), "+r" (d[27]), "+r" (d[28]), "+r" (d[29]), "+r" (d[30]), "+r" (d[31])
+      : "l" (adesc), "l" (bdesc), "r" (accumulate) : "memory");
+#endif
+}
+// V pass step: D (64 columns x 32 rows, s32) (+)= hs (u8) x vband (s8)
+__device__ __forceinline__ void tc_mma_v (int (&d)[16], uint64_t adesc, uint64_t bdesc, int accumulate)
+{
+#ifndef B200_CUDA_EMU
+  asm volatile ("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k32.s32.u8.s8 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p;\n\t}\n"
+      : "+r" (d[0]), "+r" (d[1]), "+r" (d[2]), "+r" (d[3]), "+r" (d[4]), "+r" (d[5]), "+r" (d[6]), "+r" (d[7]),
+        "+r" (d[8]), "+r" (d[9]), "+r" (d[10]), "+r" (d[11]), "+r" (d[12]), "+r" (d[13]), "+r" (d[14]), "+r" (d[15])
+      : "l" (adesc), "l" (bdesc), "r" (accumulate) : "memory");
 #endif
 }
 
-// four consecutive FIR sums -> four rounded, saturated bytes (lowest byte = first sum); the rounding constant is already
+// two consecutive FIR sums -> two rounded, saturated bytes (lowest byte = first sum); the rounding constant is already
 // in the accumulator (the extra K step)
 template <bool X4>
-__device__ __forceinline__ unsigned tc_pack4 (int a0, int a1, int a2, int a3)
+__device__ __forceinline__ unsigned short tc_pack2 (int a0, int a1)
 {
-  if (X4) return __byte_perm (pack_sat_u16x2 (a1, a0), pack_sat_u16x2 (a3, a2), 0x7531);
-  return pack_sat2 (a1 >> 6, a0 >> 6, pack_sat2 (a3 >> 6, a2 >> 6, 0u));
+  if (X4) return (unsigned short) __byte_perm (pack_sat_u16x2 (a1, a0), 0, 0x4431);
+  return (unsigned short) pack_sat2 (a1 >> 6, a0 >> 6, 0u);
+}
+
+// one output pixel from the three rounded V sums: AYUV -> ARGB (mulhi matrix) -> the output byte order
+template <bool X4>
+__device__ __forceinline__ unsigned tc_pixel (const VcsDev & P, int y, int u, int v)
+{
+  unsigned yuv = X4 ? __byte_perm (pack_sat_u16x2 (u, y), pack_sat_u16x2 (0, v), 0x7531)
+      : pack_sat2 (u >> 6, y >> 6, pack_sat2 (0, v >> 6, 0u));
+  yuv ^= 0x00808080u;
+  const int wy = prmt_s (yuv, 0x8800u), wu = prmt_s (yuv, 0x9911u), wv = prmt_s (yuv, 0xaa22u);
+  const int ty = ((wy * P.p1) >> 16) + 128;
+  const int r = ty + ((wv * P.p2) >> 16);
+  const int b = ty + ((wu * P.p3) >> 16);
+  const int gg = ty + ((wu * P.p4) >> 16) + ((wv * P.p5) >> 16);
+  const unsigned argb = pack_sat2 (r, 255, pack_sat2 (b, gg, 0u));
+  return __byte_perm (argb, 0, P.sel);
 }
 
 // ---- the kernel ------------------------------------------------------------------------------------------------------
-// One persistent CTA per SM, warp-specialised (the canonical sm_100 pipeline, with SIMT stages where a GEMM has TMA):
-//
-//   warps 0-7   PRODUCERS   stage tile k+1: Y by cp.async, prepared chroma by SIMT, tap bands -> planes[k&1]
-//   warps 8-15  CONSUMERS   tile k: H epilogue (TMEM -> bytes -> V operand), V epilogue (TMEM -> matrix -> stores)
-//   warp 16     MMA ISSUER  one lane: H pass of tile k+1 (30 MMAs), then V pass of tile k (9 MMAs)
-//
-// mbarriers:  full[2] (producers -> issuer: planes staged), empty[2] (commit of the H pass: planes free again),
-// dh_full[2] / dh_empty[2] (H accumulators of the two TMEM buffers), hs_full (consumers -> issuer: V operand written),
-// dv_full (commit of the V pass).  TMEM: 2 x 192 columns for the H pass, 96 for the V pass.
-constexpr int TC_PROD_WARPS = 8, TC_CONS_WARPS = 8;
-constexpr int TC_THREADS2 = 32 * (TC_PROD_WARPS + TC_CONS_WARPS + 1);
-constexpr int TC_VB_RING = 4;
-constexpr int TC2_OFF_BAND = 0;
-constexpr int TC2_OFF_ONES = TC2_OFF_BAND + TC_BAND_BYTES;
-constexpr int TC2_OFF_VB = TC2_OFF_ONES + TC_ONES_BYTES;
-constexpr int TC2_OFF_IMG = TC2_OFF_VB + TC_VB_RING * TC_VB_BYTES;      // 2 buffers x 3 planes
-constexpr int TC2_OFF_HS = TC2_OFF_IMG + 2 * 3 * TC_IMG_BYTES;
-constexpr int TC2_OFF_BAR = TC2_OFF_HS + 3 * TC_HS_BYTES;
-constexpr int TC2_SMEM = TC2_OFF_BAR + 128;
-constexpr int TC2_TMEM_COLS = 512;
-constexpr int TC2_DV_COL = 2 * 3 * TC_N;                                // 384: the V accumulators
-enum { TCB_FULL0 = 0, TCB_FULL1, TCB_EMPTY0, TCB_EMPTY1, TCB_DHF0, TCB_DHF1, TCB_DHE0, TCB_DHE1, TCB_HSF, TCB_DVF, TCB_COUNT };
-
-__device__ __forceinline__ void tc_bar_wait_guard (uint32_t bar, uint32_t parity)
-{
-#ifndef B200_CUDA_EMU
-  uint32_t ok, spins = 0;
-  do {
-    asm volatile ("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-        : "=r" (ok) : "r" (bar), "r" (parity) : "memory");
-    if (!ok) {
-      __nanosleep (40);                                           // a waiting warp should not compete for issue slots
-      if (++spins > (1u << 24)) __trap ();                        // a lost arrival must fail loudly, not hang the device
-    }
-  } while (!ok);
-#endif
-}
-__device__ __forceinline__ bool tc_bar_test (uint32_t bar, uint32_t parity)
-{
-#ifndef B200_CUDA_EMU
-  uint32_t ok;
-  asm volatile ("{\n\t.reg .pred p;\n\tmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-      : "=r" (ok) : "r" (bar), "r" (parity) : "memory");
-  return ok != 0;
-#else
-  return true;
-#endif
-}
-__device__ __forceinline__ void tc_bar_arrive (uint32_t bar)
-{
-#ifndef B200_CUDA_EMU
-  asm volatile ("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r" (bar) : "memory");
-#endif
-}
-
-template <bool X4, bool FULL>
-__device__ __forceinline__ void tc_v_rows (const VcsDev & P, const int (&a)[3][16], uint8_t *dst, int rows)
-{
-#pragma unroll
-  for (int i = 0; i < 14; i++) {
-    if (FULL || i < rows) {
-      unsigned yuv = X4 ? __byte_perm (pack_sat_u16x2 (a[1][i], a[0][i]), pack_sat_u16x2 (0, a[2][i]), 0x7531)
-          : pack_sat2 (a[1][i] >> 6, a[0][i] >> 6, pack_sat2 (0, a[2][i] >> 6, 0u));
-      yuv ^= 0x00808080u;
-      const int wy = prmt_s (yuv, 0x8800u), wu = prmt_s (yuv, 0x9911u), wv = prmt_s (yuv, 0xaa22u);
-      const int ty = ((wy * P.p1) >> 16) + 128;
-      const int r = ty + ((wv * P.p2) >> 16);
-      const int b = ty + ((wu * P.p3) >> 16);
-      const int gg = ty + ((wu * P.p4) >> 16) + ((wv * P.p5) >> 16);
-      const unsigned argb = pack_sat2 (r, 255, pack_sat2 (b, gg, 0u));
-      *(unsigned *) dst = __byte_perm (argb, 0, P.sel);
-    }
-    dst += P.stride_out;
-  }
-}
-
-template <int DBG>
-__global__ void __launch_bounds__ (TC_THREADS2, 1)
-vcs_l2tc_kernel (const VcsDev P, const L2tcDev L, const VcsBatch frames, int n_frames, unsigned *dbg)
+// One persistent CTA per SM walks its tiles (strip, frame, row tile); per tile:
+//   1. all eight warps stage the tile: tap bands and Y by cp.async, the up-sampled chroma by SIMT
+//   2. each warpgroup runs the H pass of its 64 columns channel by channel and writes the rounded bytes as the V pass's
+//      A operand
+//   3. each warpgroup runs the V pass of its 64 columns for the three channels, then converts and stores the pixels
+// wgmma fragment of D (m64nN): warp w of the warpgroup, lane = 4 g + t holds rows 16 w + g and 16 w + g + 8, columns
+// 8 i + 2 t and 8 i + 2 t + 1: d[4 i + 0..3] = (g, 2t), (g, 2t + 1), (g + 8, 2t), (g + 8, 2t + 1).  In the code g is fr, t is t4.
+__global__ void __launch_bounds__ (TC_THREADS, 1)
+vcs_l2tc_kernel (const VcsDev P, const L2tcDev L, const VcsBatch frames, int n_frames)
 {
 #ifndef B200_CUDA_EMU
   extern __shared__ __align__ (128) uint8_t sm[];
   const int tid = threadIdx.x, lane = tid & 31;
   const int warp = __shfl_sync (0xffffffffu, tid >> 5, 0);
+  const int wg = warp >> 2, fr = lane >> 2, t4 = lane & 3;      // fr, t4: row group / pair of a wgmma fragment
   const uint32_t s_base = tc_smem_u32 (sm);
-  const uint32_t s_band = s_base + TC2_OFF_BAND, s_ones = s_base + TC2_OFF_ONES, s_vb = s_base + TC2_OFF_VB,
-      s_img = s_base + TC2_OFF_IMG, s_hs = s_base + TC2_OFF_HS, s_bar = s_base + TC2_OFF_BAR, s_tptr = s_bar + 8 * TCB_COUNT;
-  auto bar = [&] (int i) { return s_bar + 8u * (uint32_t) i; };
+  const uint32_t s_band = s_base + TC_OFF_BAND, s_ones = s_base + TC_OFF_ONES, s_vb = s_base + TC_OFF_VB,
+      s_img = s_base + TC_OFF_IMG, s_hs = s_base + TC_OFF_HS;
 
-  if (tid == 0) {
-    const int counts[TCB_COUNT] = {TC_PROD_WARPS, TC_PROD_WARPS, 1, 1, 1, 1, TC_CONS_WARPS, TC_CONS_WARPS, TC_CONS_WARPS, 1};
-    for (int i = 0; i < TCB_COUNT; i++)
-      asm volatile ("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r" (bar (i)), "r" (counts[i]) : "memory");
-    asm volatile ("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == TC_PROD_WARPS + TC_CONS_WARPS) {
-    asm volatile ("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r" (s_tptr), "r" (TC2_TMEM_COLS) : "memory");
-    asm volatile ("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  for (int i = tid; i < TC_ONES_BYTES / 16; i += TC_THREADS2)
-    *(uint4 *) (sm + TC2_OFF_ONES + 16 * i) = make_uint4 (0x01010101u, 0x01010101u, 0x01010101u, 0x01010101u);
-  tc_fence_async_smem ();
-  tc_fence_before ();
-  __syncthreads ();
-  tc_fence_after ();
-  const uint32_t tmem = *(volatile uint32_t *) (sm + TC2_OFF_BAR + 8 * TCB_COUNT);
+  for (int i = tid; i < TC_ONES_BYTES / 16; i += TC_THREADS)
+    *(uint4 *) (sm + TC_OFF_ONES + 16 * i) = make_uint4 (0x01010101u, 0x01010101u, 0x01010101u, 0x01010101u);
 
   const int per_strip = n_frames * L.row_tiles;
   const int n_tiles = L.strips * per_strip;
@@ -278,34 +204,35 @@ vcs_l2tc_kernel (const VcsDev P, const L2tcDev L, const VcsBatch frames, int n_f
     if ((unsigned) (f + 1) * (unsigned) L.row_tiles <= rem) f++;
     rt = (int) (rem - (unsigned) f * (unsigned) L.row_tiles);
   };
+  // descriptors differ only in their start-address field (bits 0..13, units of 16 bytes): base descriptor + offset.
+  // Warpgroup wg's 64 rows of an A operand start 64 rows = 8 core matrices (1 KB) further.
+  const uint64_t d_band = tc_desc (s_band + 1024u * wg, TC_BAND_LBO, 128), d_ones = tc_desc (s_ones, TC_BAND_LBO, 128);
+  const uint64_t d_img = tc_desc (s_img, TC_IMG_LBO, 128), d_hs = tc_desc (s_hs + 1024u * wg, TC_HS_LBO, 128);
+  const uint64_t d_vb = tc_desc (s_vb, TC_VB_LBO, 128);
 
-  if (warp < TC_PROD_WARPS) {
-    // ================================================================ PRODUCERS
-    const int crows = P.ih >> 1;
-    const unsigned selU = P.u_index ? 0x7531u : 0x6420u, selV = P.u_index ? 0x6420u : 0x7531u;
-    const unsigned nselU = P.u_index ? 0x5321u : 0x4321u, nselV = P.u_index ? 0x4321u : 0x5321u;
-    int prev_strip = -1;
-    for (int k = 0; k < my_tiles; k++) {
-      int strip, f, rt;
-      tile_of (k, strip, f, rt);
-      const int buf = k & 1, use = k >> 1;
-      if (use > 0) tc_bar_wait_guard (bar (TCB_EMPTY0 + buf), (use - 1) & 1);          // H pass of tile k-2 has read these planes
+  const int crows = P.ih >> 1;
+  const unsigned selU = P.u_index ? 0x7531u : 0x6420u, selV = P.u_index ? 0x6420u : 0x7531u;
+  const unsigned nselU = P.u_index ? 0x5321u : 0x4321u, nselV = P.u_index ? 0x4321u : 0x5321u;
+  int prev_strip = -1;
+  for (int k = 0; k < my_tiles; k++) {
+    int strip, f, rt;
+    tile_of (k, strip, f, rt);
+    const int x0 = strip * TC_TW, oy0 = rt * TC_TH;
+    __syncthreads ();                                              // both warpgroups are done with the previous tile's operands
+    // ================================================================ 1. staging
+    {
       if (strip != prev_strip) {
-        // the band is single-buffered: the H pass of tile k-1 must have finished with the old one
-        if (k > 0) tc_bar_wait_guard (bar (TCB_EMPTY0 + (buf ^ 1)), ((k - 1) >> 1) & 1);
         const uint8_t *src = L.band + (size_t) strip * TC_BAND_BYTES;
-        for (int i = tid; i < TC_BAND_BYTES / 16; i += 32 * TC_PROD_WARPS) tc_cp16 (s_band + 16 * i, src + 16 * i);
+        for (int i = tid; i < TC_BAND_BYTES / 16; i += TC_THREADS) tc_cp16 (s_band + 16 * i, src + 16 * i);
         prev_strip = strip;
       }
       const uint8_t *__restrict__ in = frames.in[f];
       const uint8_t *__restrict__ plane_y = in + P.off_y;
       const uint8_t *__restrict__ plane_c = in + P.off_c;
-      const int x0 = strip * TC_TW, oy0 = rt * TC_TH;
       const int X0 = 2 * x0 - TC_X_LEAD, R0 = 2 * oy0 - 3;
-      const uint32_t img = s_img + buf * 3 * TC_IMG_BYTES;
-      uint8_t *img_u = sm + TC2_OFF_IMG + buf * 3 * TC_IMG_BYTES + TC_IMG_BYTES, *img_v = img_u + TC_IMG_BYTES;
-      if (tid < TC_VB_BYTES / 16)
-        tc_cp16 (s_vb + (k % TC_VB_RING) * TC_VB_BYTES + 16 * tid, L.vband + (size_t) rt * TC_VB_BYTES + 16 * tid);
+      const uint32_t img = s_img;
+      uint8_t *img_u = sm + TC_OFF_IMG + TC_IMG_BYTES, *img_v = img_u + TC_IMG_BYTES;
+      if (tid < TC_VB_BYTES / 16) tc_cp16 (s_vb + 16 * tid, L.vband + (size_t) rt * TC_VB_BYTES + 16 * tid);
       // Y: a warp takes lines w, w + 8, ...; lanes 0..17 one 16-byte chunk each
       {
         const int x = X0 + 16 * lane;
@@ -392,137 +319,74 @@ vcs_l2tc_kernel (const VcsDev P, const L2tcDev L, const VcsBatch frames, int n_f
         }
       }
       tc_cp_wait ();
-      tc_fence_async_smem ();
-      __syncwarp ();
-      if (lane == 0) tc_bar_arrive (bar (TCB_FULL0 + buf));
+      tc_fence_async_smem ();                                      // generic-proxy writes -> visible to wgmma
+      __syncthreads ();
     }
-  } else if (warp < TC_PROD_WARPS + TC_CONS_WARPS) {
-    // ================================================================ CONSUMERS
-    const int cw = warp - TC_PROD_WARPS, qd = cw & 3, hf = cw >> 2;
-    const int col = 32 * qd + lane;
-    const uint32_t lane_base = tmem + ((uint32_t) (32 * qd) << 16);
-    for (int k = 0; k < my_tiles; k++) {
-      int strip, f, rt;
-      tile_of (k, strip, f, rt);
-      const int acc = k & 1, use = k >> 1;
-      // ---------------- H epilogue: 32 lines of one column per thread and channel
-      tc_bar_wait_guard (bar (TCB_DHF0 + acc), use & 1);
-      tc_fence_after ();
-      const bool hx4 = __ldg (L.hx4 + strip) != 0;
+    // ================================================================ 2. H pass, one channel at a time
+    const bool hx4 = __ldg (L.hx4 + strip) != 0;                  // block-uniform
 #pragma unroll 1
-      for (int ch = 0; ch < 3; ch++) {
-        int v[32];
-        const uint32_t ta = lane_base + acc * 3 * TC_N + ch * TC_N + 32 * hf;
-        TC_LD16 (v, ta);
-        TC_LD16 ((v + 16), (ta + 16));
-        tc_ld_wait ();
-        if (DBG == 1 && dbg && blockIdx.x == 0 && k == 0) {
+    for (int ch = 0; ch < 3; ch++) {
+      int d[32];
 #pragma unroll
-          for (int i = 0; i < 32; i++) dbg[(ch * 128 + col) * 64 + 32 * hf + i] = (unsigned) v[i];
-        }
-        uint4 w0, w1;
-        if (hx4) {
-          w0.x = tc_pack4<true> (v[0], v[1], v[2], v[3]); w0.y = tc_pack4<true> (v[4], v[5], v[6], v[7]);
-          w0.z = tc_pack4<true> (v[8], v[9], v[10], v[11]); w0.w = tc_pack4<true> (v[12], v[13], v[14], v[15]);
-          w1.x = tc_pack4<true> (v[16], v[17], v[18], v[19]); w1.y = tc_pack4<true> (v[20], v[21], v[22], v[23]);
-          w1.z = tc_pack4<true> (v[24], v[25], v[26], v[27]); w1.w = tc_pack4<true> (v[28], v[29], v[30], v[31]);
-        } else {
-          w0.x = tc_pack4<false> (v[0], v[1], v[2], v[3]); w0.y = tc_pack4<false> (v[4], v[5], v[6], v[7]);
-          w0.z = tc_pack4<false> (v[8], v[9], v[10], v[11]); w0.w = tc_pack4<false> (v[12], v[13], v[14], v[15]);
-          w1.x = tc_pack4<false> (v[16], v[17], v[18], v[19]); w1.y = tc_pack4<false> (v[20], v[21], v[22], v[23]);
-          w1.z = tc_pack4<false> (v[24], v[25], v[26], v[27]); w1.w = tc_pack4<false> (v[28], v[29], v[30], v[31]);
-        }
-        uint8_t *hs = sm + TC2_OFF_HS + ch * TC_HS_BYTES + (2 * hf) * TC_HS_LBO + col * 16;
-        *(uint4 *) hs = w0;
-        *(uint4 *) (hs + TC_HS_LBO) = w1;
-      }
-      tc_fence_before ();
-      tc_fence_async_smem ();
-      __syncwarp ();
-      if (lane == 0) { tc_bar_arrive (bar (TCB_DHE0 + acc)); tc_bar_arrive (bar (TCB_HSF)); }
-      // ---------------- V epilogue: 14 rows of one column per thread
-      tc_bar_wait_guard (bar (TCB_DVF), k & 1);
-      tc_fence_after ();
-      {
-        const int x0 = strip * TC_TW, oy0 = rt * TC_TH, ox = x0 + col, r0 = 14 * hf;
-        int a[3][16];
-        const uint32_t ta = lane_base + TC2_DV_COL + r0;
-        TC_LD16 (a[0], ta);
-        TC_LD16 (a[1], (ta + TC_VROWS));
-        TC_LD16 (a[2], (ta + 2 * TC_VROWS));
-        tc_ld_wait ();
-        tc_fence_before ();                                        // the next V pass may overwrite the accumulators once hs_full comes
-        const int rows = min (min (TC_TH, P.oh - oy0) - r0, 14);
-        if (ox < P.ow && rows > 0) {
-          uint8_t *dst = frames.out[f] + P.off_out + (size_t) (oy0 + r0) * P.stride_out + (size_t) ox * 4u;
-          const bool vx4 = __ldg (L.vx4 + rt) != 0;              // warp-uniform: branches, not predicates
-          if (rows == 14) { if (vx4) tc_v_rows<true, true> (P, a, dst, 14); else tc_v_rows<false, true> (P, a, dst, 14); }
-          else { if (vx4) tc_v_rows<true, false> (P, a, dst, rows); else tc_v_rows<false, false> (P, a, dst, rows); }
-        }
-      }
-    }
-  } else if (lane == 0) {
-    // ================================================================ MMA ISSUER (one lane)
-    constexpr uint32_t IDESC_H = tc_idesc (1, 0, TC_N, 128), IDESC_V = tc_idesc (0, 1, TC_VROWS, 128);
-    // Both passes are issued from one lane in whatever order their inputs become ready: the H pass of tile k+1 must not
-    // wait behind the V pass of tile k (that one waits for the consumers), nor the other way round (the H pass waits for
-    // the producers).  The H pass runs at most one tile ahead (two TMEM / plane buffers).
-    // descriptors differ only in their start-address field (bits 0..13, units of 16 bytes): base descriptor + offset
-    const uint64_t d_band = tc_desc (s_band, TC_BAND_LBO, 128), d_ones = tc_desc (s_ones, TC_BAND_LBO, 128);
-    const uint64_t d_img = tc_desc (s_img, TC_IMG_LBO, 128), d_hs = tc_desc (s_hs, TC_HS_LBO, 128);
-    const uint64_t d_vb = tc_desc (s_vb, TC_VB_LBO, 128);
-    auto issue_h_ch = [&] (int k, int ch) {                       // one channel of the H pass: 9 K steps + the rounding step
-      const int buf = k & 1;
-      const uint64_t img = d_img + (uint64_t) (((buf * 3 + ch) * TC_IMG_BYTES) >> 4);
-      const uint32_t acc = tmem + buf * 3 * TC_N + ch * TC_N;
+      for (int i = 0; i < 32; i++) d[i] = 0;
+      const uint64_t img = d_img + (uint64_t) ((ch * TC_IMG_BYTES) >> 4);
+      tc_fence_regs (d);
+      tc_wg_fence ();
 #pragma unroll
       for (int s = 0; s < TC_CHUNKS / 2; s++)
-        tc_mma (acc, d_band + (uint64_t) ((2 * s * TC_BAND_LBO) >> 4), img + (uint64_t) ((2 * s * TC_IMG_LBO) >> 4), IDESC_H, s > 0);
-      tc_mma (acc, d_band + (uint64_t) ((TC_CHUNKS * TC_BAND_LBO) >> 4), d_ones, IDESC_H, 1);
-      if (ch == 2) {
-        tc_commit (bar (TCB_EMPTY0 + buf));
-        tc_commit (bar (TCB_DHF0 + buf));
+        tc_mma_h (d, d_band + (uint64_t) ((2 * s * TC_BAND_LBO) >> 4), img + (uint64_t) ((2 * s * TC_IMG_LBO) >> 4), s > 0);
+      tc_mma_h (d, d_band + (uint64_t) ((TC_CHUNKS * TC_BAND_LBO) >> 4), d_ones, 1);
+      tc_wg_commit_wait ();
+      tc_fence_regs (d);
+      // rows = output columns j, columns = staged lines l: the pair (l, l + 1) is two adjacent bytes of hs row j
+      uint8_t *hs = sm + TC_OFF_HS + ch * TC_HS_BYTES + (64 * wg + 16 * (warp & 3) + fr) * 16;
+#pragma unroll
+      for (int i = 0; i < 8; i++) {
+        const int l = 8 * i + 2 * t4;
+        uint8_t *p = hs + (l >> 4) * TC_HS_LBO + (l & 15);
+        if (hx4) {
+          *(unsigned short *) p = tc_pack2<true> (d[4 * i], d[4 * i + 1]);
+          *(unsigned short *) (p + 8 * 16) = tc_pack2<true> (d[4 * i + 2], d[4 * i + 3]);
+        } else {
+          *(unsigned short *) p = tc_pack2<false> (d[4 * i], d[4 * i + 1]);
+          *(unsigned short *) (p + 8 * 16) = tc_pack2<false> (d[4 * i + 2], d[4 * i + 3]);
+        }
       }
-    };
-    auto issue_v = [&] (int k) {
-      tc_fence_after ();
-      const uint64_t vb = d_vb + (uint64_t) (((k % TC_VB_RING) * TC_VB_BYTES) >> 4);
+    }
+    tc_fence_async_smem ();
+    __syncthreads ();
+    // ================================================================ 3. V pass, the three channels together
+    {
+      int a[3][16];
+#pragma unroll
+      for (int ch = 0; ch < 3; ch++)
+#pragma unroll
+        for (int i = 0; i < 16; i++) a[ch][i] = 0;
+      tc_fence_regs (a[0]); tc_fence_regs (a[1]); tc_fence_regs (a[2]);
+      tc_wg_fence ();
 #pragma unroll
       for (int ch = 0; ch < 3; ch++) {
         const uint64_t hs = d_hs + (uint64_t) ((ch * TC_HS_BYTES) >> 4);
-        const uint32_t acc = tmem + TC2_DV_COL + ch * TC_VROWS;
 #pragma unroll
         for (int s = 0; s < TC_N / 32; s++)
-          tc_mma (acc, hs + (uint64_t) ((2 * s * TC_HS_LBO) >> 4), vb + (uint64_t) ((2 * s * TC_VB_LBO) >> 4), IDESC_V, s > 0);
-        tc_mma (acc, d_ones, vb + (uint64_t) ((2 * (TC_N / 32) * TC_VB_LBO) >> 4), IDESC_V, 1);
+          tc_mma_v (a[ch], hs + (uint64_t) ((2 * s * TC_HS_LBO) >> 4), d_vb + (uint64_t) ((2 * s * TC_VB_LBO) >> 4), s > 0);
+        tc_mma_v (a[ch], d_ones, d_vb + (uint64_t) ((2 * (TC_N / 32) * TC_VB_LBO) >> 4), 1);
       }
-      tc_commit (bar (TCB_DVF));
-    };
-    // The tensor pipe runs its MMAs in issue order, so the short V pass (consumers wait for it) is looked at between the
-    // three channel-sized bites of the long H pass instead of after all of it.
-    int nh = 0, hch = 0, nv = 0;                                  // hch: channels of H pass nh already issued
-    uint32_t idle = 0;
-    while (nv < my_tiles) {
-      bool progressed = false;
-      if (nv < nh && tc_bar_test (bar (TCB_HSF), nv & 1)) { issue_v (nv); nv++; progressed = true; }
-      if (nh < my_tiles && nh <= nv + 1) {
-        const int buf = nh & 1, use = nh >> 1;
-        if (hch > 0 || (tc_bar_test (bar (TCB_FULL0 + buf), use & 1) && (use == 0 || tc_bar_test (bar (TCB_DHE0 + buf), (use - 1) & 1)))) {
-          if (hch == 0) tc_fence_after ();
-          issue_h_ch (nh, hch);
-          if (++hch == 3) { hch = 0; nh++; }
-          progressed = true;
-        }
+      tc_wg_commit_wait ();
+      tc_fence_regs (a[0]); tc_fence_regs (a[1]); tc_fence_regs (a[2]);
+      // rows = output columns, columns = output rows of the tile
+      const bool vx4 = __ldg (L.vx4 + rt) != 0;
+      uint8_t *out = frames.out[f] + P.off_out;
+#pragma unroll
+      for (int e = 0; e < 16; e++) {
+        const int ox = x0 + 64 * wg + 16 * (warp & 3) + fr + ((e & 2) ? 8 : 0);
+        const int r = 8 * (e >> 2) + 2 * t4 + (e & 1);
+        if (r < TC_TH && oy0 + r < P.oh && ox < P.ow)
+          *(unsigned *) (out + (size_t) (oy0 + r) * P.stride_out + (size_t) ox * 4u) =
+              vx4 ? tc_pixel<true> (P, a[0][e], a[1][e], a[2][e]) : tc_pixel<false> (P, a[0][e], a[1][e], a[2][e]);
       }
-      if (progressed) idle = 0;
-      else if (++idle > (1u << 27)) __trap ();
     }
   }
-
-  tc_fence_before ();
-  __syncthreads ();
-  if (warp == TC_PROD_WARPS + TC_CONS_WARPS)
-    asm volatile ("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r" (tmem), "r" (TC2_TMEM_COLS) : "memory");
 #endif
 }
 
@@ -608,28 +472,19 @@ inline int prepare_l2tc (const L2tcTables & t, L2tcState * st)
   return B200_OK;
 }
 
-inline int launch_l2tc (const VcsDev & d, const L2tcState & st, const VcsBatch & batch, int n, cudaStream_t stream,
-    unsigned *dbg = nullptr, int dbg_mode = 0)
+inline int launch_l2tc (const VcsDev & d, const L2tcState & st, const VcsBatch & batch, int n, cudaStream_t stream)
 {
   int rc;
   int dev = 0;
   B200_CUDA_TRY (cudaGetDevice (&dev));
   const int tiles = st.dev.strips * st.dev.row_tiles * n;
   const int grid = min (tiles, sm_count (dev));
-  if (dbg_mode == 1) {
-    if ((rc = allow_max_dyn_smem (vcs_l2tc_kernel<1>)) != B200_OK) return rc;
-    vcs_l2tc_kernel<1> <<<grid, TC_THREADS2, TC2_SMEM, stream>>> (d, st.dev, batch, n, dbg);
-  } else if (dbg_mode == 2) {
-    if ((rc = allow_max_dyn_smem (vcs_l2tc_kernel<2>)) != B200_OK) return rc;
-    vcs_l2tc_kernel<2> <<<grid, TC_THREADS2, TC2_SMEM, stream>>> (d, st.dev, batch, n, dbg);
-  } else {
-    static bool attr_done[16] = {false};
-    if (!attr_done[dev & 15]) {
-      if ((rc = allow_max_dyn_smem (vcs_l2tc_kernel<0>)) != B200_OK) return rc;
-      attr_done[dev & 15] = true;
-    }
-    vcs_l2tc_kernel<0> <<<grid, TC_THREADS2, TC2_SMEM, stream>>> (d, st.dev, batch, n, nullptr);
+  static bool attr_done[16] = {false};
+  if (!attr_done[dev & 15]) {
+    if ((rc = allow_max_dyn_smem (vcs_l2tc_kernel)) != B200_OK) return rc;
+    attr_done[dev & 15] = true;
   }
+  vcs_l2tc_kernel <<<grid, TC_THREADS, TC_SMEM, stream>>> (d, st.dev, batch, n);
   B200_CUDA_TRY (cudaGetLastError ());
   return B200_OK;
 }

@@ -1,5 +1,5 @@
 // gstreamer_b200/csrc/vcs_lanczos2.cuh — specialised fused kernel for the headline shape class
-// (product code, sm_100a): 4:2:0 semi-planar -> packed RGB, exact 2:1 reduction in both
+// (product code, sm_90a): 4:2:0 semi-planar -> packed RGB, exact 2:1 reduction in both
 // directions with the 8-tap filters the reference derives for it (lanczos and every other
 // 8-tap/2:1 method), h-cosited chroma, all input lines consumed in order.
 //
@@ -100,7 +100,7 @@ __device__ __forceinline__ int prmt_s (unsigned a, unsigned sel)      // prmt.b3
 #endif
 }
 // acc >> 6 (arithmetic).  SHF runs at half rate on the ALU pipe; IMAD.HI would be a quarter-rate
-// alternative on sm_100a (profiles/r01_ubench_sm100a.txt), so the plain shift stays.
+// alternative, so the plain shift stays.
 __device__ __forceinline__ int sra6 (int acc) { return acc >> 6; }
 // d = { c[15:0], sat_u8(a), sat_u8(b) }  (b in the lowest byte)
 __device__ __forceinline__ unsigned pack_sat2 (int a, int b, unsigned c)
@@ -130,17 +130,13 @@ __device__ __forceinline__ unsigned pack_sat_u16x2 (int a, int b)
 // 4 outputs from 16 aligned bytes w0..w3: outputs 0,1 read words 0..2, outputs 2,3 words 1..3
 #define L2_FIR4(o0, o1, o2, o3, w0, w1, w2, w3, T, INIT)                                       \
   do {                                                                                         \
-    if (ABL & L2_FIR_BIT) { o0 = (w0) + T[0].x; o1 = (w1) + T[1].x; o2 = (w2) + T[2].x; o3 = (w3) + INIT; break; } \
     o0 = dp4a_u8s8 (w2, T[0].z, dp4a_u8s8 (w1, T[0].y, dp4a_u8s8 (w0, T[0].x, INIT)));         \
     o1 = dp4a_u8s8 (w2, T[1].y, dp4a_u8s8 (w1, T[1].x, dp4a_u8s8 (w0, T[0].w, INIT)));         \
     o2 = dp4a_u8s8 (w3, T[2].x, dp4a_u8s8 (w2, T[1].w, dp4a_u8s8 (w1, T[1].z, INIT)));         \
     o3 = dp4a_u8s8 (w3, T[2].w, dp4a_u8s8 (w2, T[2].z, dp4a_u8s8 (w1, T[2].y, INIT)));         \
   } while (0)
 
-// ABL != 0: NON-PARITY ablation builds for tools/l2lab.cu (which stage costs what, measured instead of counted); the
-// product only ever instantiates ABL = 0.  Bits: 1 no chroma preparation, 2 no H FIR, 4 no V phase, 8 no H phase,
-// 16 no matrix, 32 no V FIR.
-template <bool ALPHA_OPAQUE, int MINB, int TH, int NWC, bool X4 = false, int ABL = 0>
+template <bool ALPHA_OPAQUE, int MINB, int TH, int NWC, bool X4 = false>
 __global__ void __launch_bounds__ (L2_THREADS, MINB)
 vcs_lanczos2_kernel (const VcsDev P, const Lanczos2Dev L, const VcsBatch frames)
 {
@@ -162,10 +158,8 @@ vcs_lanczos2_kernel (const VcsDev P, const Lanczos2Dev L, const VcsBatch frames)
   // Tiles that touch no frame border skip every clamp (line / chroma-row / column indices and the
   // "no chroma sample to the right" fix-up): warp-uniform choice between two instantiations.
   const bool edge_tile = R0 < 0 || R0 + 4 * L2_NG > P.ih || x0 == 0 || x0 + L2_TW + 4 >= P.ow;
-#define L2_FIR_BIT 2
   auto h_phase = [&] (auto edge_tag) {
     constexpr bool EDGE = decltype (edge_tag)::value;
-    if (ABL & 8) return;
     constexpr bool H4 = X4 && !EDGE;                             // interior tiles only: no folded taps there
     constexpr int HINIT = H4 ? 128 : 32;
     const int4 *__restrict__ htab = H4 ? L.htab4 : L.htab;
@@ -203,19 +197,14 @@ vcs_lanczos2_kernel (const VcsDev P, const Lanczos2Dev L, const VcsBatch frames)
         un = __byte_perm (ue, un, 0x4321);
         vn = __byte_perm (ve, vn, 0x4321);
       }
-      const unsigned uo = (ABL & 1) ? un : avg_ceil4 (ue, un), vo = (ABL & 1) ? vn : avg_ceil4 (ve, vn);
+      const unsigned uo = avg_ceil4 (ue, un), vo = avg_ceil4 (ve, vn);
       ulo[k] = __byte_perm (ue, uo, 0x5140); uhi[k] = __byte_perm (ue, uo, 0x7362);
       vlo[k] = __byte_perm (ve, vo, 0x5140); vhi[k] = __byte_perm (ve, vo, 0x7362);
     }
     // vertical pairs (4m+1,4m+2) on rows (a,b) and (4m+3,4m+4) on rows (b,c):
     // (3x+y+2)>>2 == avg_ceil (x, avg_floor (x,y))   (video-orc.orc:2705-2735)
     unsigned U[4][2], V[4][2];
-    if (ABL & 1) {
-#pragma unroll
-      for (int r = 0; r < 4; r++) {
-        U[r][0] = ulo[(r + 1) >> 1]; U[r][1] = uhi[(r + 1) >> 1]; V[r][0] = vlo[(r + 1) >> 1]; V[r][1] = vhi[(r + 1) >> 1];
-      }
-    } else {
+    {
       unsigned f;
       f = avg_floor4 (ulo[0], ulo[1]); U[0][0] = avg_ceil4 (ulo[0], f); U[1][0] = avg_ceil4 (ulo[1], f);
       f = avg_floor4 (uhi[0], uhi[1]); U[0][1] = avg_ceil4 (uhi[0], f); U[1][1] = avg_ceil4 (uhi[1], f);
@@ -265,10 +254,7 @@ vcs_lanczos2_kernel (const VcsDev P, const Lanczos2Dev L, const VcsBatch frames)
   }
   };
   if (edge_tile) h_phase (std::true_type {}); else h_phase (std::false_type {});
-#undef L2_FIR_BIT
-#define L2_FIR_BIT 32
   __syncthreads ();
-  if (ABL & 4) return;
 
   // ---------------------------------------------------------------- V phase
   // a warp owns output rows oy0+4q .. +3 for all columns of the tile.  The taps-times-4 choice is warp-uniform and taken
@@ -321,7 +307,7 @@ vcs_lanczos2_kernel (const VcsDev P, const Lanczos2Dev L, const VcsBatch frames)
           int al = 255;
           if (!ALPHA_OPAQUE) al = fir_round_u8 ((int) (short) (ah * vs[i]));
           // ARGB bytes in one word, then the output format's byte order
-          const unsigned argb = (ABL & 16) ? yuv : pack_sat2 (r, al, pack_sat2 (b, gg, 0u));
+          const unsigned argb = pack_sat2 (r, al, pack_sat2 (b, gg, 0u));
           *(unsigned *) (rowp[i] + 128 * k) = __byte_perm (argb, 0, P.sel);
         }
       }
@@ -334,7 +320,6 @@ vcs_lanczos2_kernel (const VcsDev P, const Lanczos2Dev L, const VcsBatch frames)
       else v_rows (std::false_type {}, q);
     }
   }
-#undef L2_FIR_BIT
 }
 
 // ------------------------------------------------------------------------------------ host side
@@ -445,7 +430,7 @@ inline int prepare_lanczos2 (const Lanczos2Tables & t, const VcsDev & d, Lanczos
   st->dev.alpha_opaque = t.alpha_opaque;
   st->dev.htab4 = st->dev.htab; st->dev.vtab4 = st->dev.vtab; st->dev.v4 = nullptr;
   const char *x4e = getenv ("B200_L2_X4");        // tuning knob: "0" keeps the plain tables
-  if (t.x4_ok && !(x4e && x4e[0] == '0')) {      // measured 0.8 % faster than the plain tables (profiles/r02_first_bench_x4.json)
+  if (t.x4_ok && !(x4e && x4e[0] == '0')) {      // the taps x 4 tables are the default; B200_L2_X4=0 selects the plain ones
     int *h4 = nullptr, *v4 = nullptr;
     if ((rc = upload (&h4, t.htab4.data (), t.htab4.size ())) != B200_OK) return rc;
     if ((rc = upload (&v4, t.vtab4.data (), t.vtab4.size ())) != B200_OK) return rc;
@@ -456,7 +441,7 @@ inline int prepare_lanczos2 (const Lanczos2Tables & t, const VcsDev & d, Lanczos
   }
   {
     const char *e = getenv ("B200_L2_VARIANT");      // tuning knob (0..3), see launch_lanczos2
-    st->variant = e ? atoi (e) : 3;        // 120x60 tiles, 4 CTAs/SM measured fastest (profiles/)
+    st->variant = e ? atoi (e) : 3;        // 120x60 tiles, 4 CTAs/SM
   }
   return B200_OK;
 }

@@ -1,11 +1,10 @@
-// gstreamer_b200/csrc/vcs_lanczos2_v2.cuh — second form of the headline kernel (product code, sm_100a).
+// gstreamer_b200/csrc/vcs_lanczos2_v2.cuh — second form of the headline kernel (product code, sm_90a).
 //
 // Same tile, same two phases and the same arithmetic as vcs_lanczos2_kernel<true, 4, 60, 1, true> (vcs_lanczos2.cuh, which
 // stays the fallback for every plan this one does not take); what changes is what the SASS histogram of that kernel showed
-// to be overhead (profiles/r02_l2_ablation_*: the kernel is bound by the issue slots and the integer pipe, 414 instructions
-// per H item and 133 per four output pixels of the V phase):
+// to be overhead (the kernel is bound by the issue slots and the integer pipe):
 //
-//  * interior tiles (no frame border in reach: 78 % of the tiles of a 4K frame) have ONE set of taps for every column - the
+//  * interior tiles (no frame border in reach: most tiles of a 4K frame) have ONE set of taps for every column - the
 //    plan proves it on the host - so the taps are kernel constants (constant-bank operands of IDP.4A): no table loads, twelve
 //    registers less
 //  * chroma words are built shifted by one pixel ([o0 e1 o1 e2] instead of [e0 o0 e1 o1]; the same PRMTs with the shifted
@@ -353,9 +352,9 @@ vcs_lanczos2_v2_kernel (const VcsDev P, const Lanczos2Dev L, const Lanczos2V2Dev
       }
     }
   };
-  // Two more things were built, measured or checked, and dropped (profiles/r02_l2_v2_lab.txt): (1) packing the 24 left-over
+  // Two more things were built, measured or checked, and dropped: (1) packing the 24 left-over
   // columns of the tile's 15 row groups into 12 full warp passes instead of 15 three-quarter-full ones - the packed passes'
-  // per-lane row pointers and indices cost more than the three passes saved (6.52 against 6.46 us/frame); (2) running the
+  // per-lane row pointers and indices cost more than the three passes saved; (2) running the
   // left / right border tiles on the constant taps over edge-REPLICATED samples - the reference folds its edge taps in
   // double precision BEFORE quantising them, so the folded integer taps are not the uniform integer taps summed over the
   // replicated positions (column 1 of the bench shape: -3 8 28 28 7 -3 -1 against -4 8 28 28 8 -3 -1): not bit-exact.
@@ -465,7 +464,7 @@ inline int launch_lanczos2_v2 (const VcsDev & d, const Lanczos2State & st, const
     }
   }
   switch (d.sel) {
-    // (prefetching the next item's loads measured slower: 6.87 against 6.56 us/frame, profiles/r02_l2_v2_lab.txt)
+    // (prefetching the next item's loads was tried: slower)
     case 0x0123u: return launch_lanczos2_v2_sel<0x0123, 0> (d, st, v2, batch, n, stream);   // BGRA / BGRx
     case 0x0321u: return launch_lanczos2_v2_sel<0x0321, 0> (d, st, v2, batch, n, stream);   // RGBA / RGBx
     default: return launch_lanczos2_v2_sel<-1, 0> (d, st, v2, batch, n, stream);

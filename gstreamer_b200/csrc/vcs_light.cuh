@@ -1,5 +1,5 @@
 // gstreamer_b200/csrc/vcs_light.cuh — fused kernel for the element's DEFAULT configuration class
-// (product code, sm_100a): 4:2:0 semi-planar -> packed RGB where each axis is either untouched /
+// (product code, sm_90a): 4:2:0 semi-planar -> packed RGB where each axis is either untouched /
 // nearest (PASS_COPY) or bilinear (PASS_2TAP), horizontal pass first.  BASELINE config C1
 // (1920x1080 NV12 -> 1280x720 BGRA, method=bilinear) lands here.
 //

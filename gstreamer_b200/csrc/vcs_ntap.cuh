@@ -1,5 +1,5 @@
 // gstreamer_b200/csrc/vcs_ntap.cuh — fused kernel for n-tap filters at ANY ratio (product code,
-// sm_100a): 4:2:0 semi-planar -> packed RGB where at least one axis runs the reference's n-tap FIR
+// sm_90a): 4:2:0 semi-planar -> packed RGB where at least one axis runs the reference's n-tap FIR
 // (lanczos / cubic / sinc / linear-as-n-tap, video_scale_h_ntap_u8 + video_scale_v_ntap_u8) and the
 // other one too or is untouched; horizontal pass first.  The exact-2:1 8-tap case has its own
 // kernel (vcs_lanczos2.cuh); this one takes every other size, e.g. 1080p -> 720p or 4K -> 720p.

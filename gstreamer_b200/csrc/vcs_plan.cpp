@@ -405,7 +405,7 @@ void light_geometry (VcsPlan * p)
   if (p->v.mode == PASS_2TAP) for (int16_t c : p->v.coef) if (c < 0 || c > 256) return;
   const int ow = p->out.width, oh = p->out.height, tw = 128;
   const char *env_th = getenv ("B200_LIGHT_TH");              // tuning aid
-  static const int heights[] = {32, 16, 8, 4, 2, 1};              // 32 rows measured best on C1 (4.77 us vs 5.67 at 16)
+  static const int heights[] = {32, 16, 8, 4, 2, 1};              // 32 rows first: fewest CTAs on C1
   for (int hi = 0; hi < 6; hi++) {
     const int th = (env_th && hi == 0) ? atoi (env_th) : heights[hi];
     int max_rows = 0, max_cols = 0;

@@ -1,6 +1,6 @@
 // gstreamer_b200/csrc/vcs_plan.h — host-side per-caps plan of the convert+scale path.
 //
-// Product code.  This is the B200 build's equivalent of the one-time setup the
+// Product code.  This is the CUDA build's equivalent of the one-time setup the
 // reference does in gst_video_converter_new_with_pool()/chain_*()
 // (gst-libs/gst/video/video-converter.c:2421, :852-2112): instead of a chain of
 // line caches it produces flat tables the fused kernels index directly.

@@ -1,6 +1,6 @@
 // gstreamer_b200/csrc/vcs_planes.cuh — YUV -> same YUV family (NV12->NV12, NV21->NV21, I420/YV12 ->
 // I420/YV12) and packed RGB -> the same packed RGB (one plane of 4-byte pixels, opt-in): the reference's
-// plane-scaling fast path (product code, sm_100a).
+// plane-scaling fast path (product code, sm_90a).
 //
 //   convert_scale_planes            gst-libs/gst/video/video-converter.c:7757-7769
 //   setup_scale                     :7958-8245  (which kernel each plane gets; built on the host, vcs_plan.cpp)
@@ -212,8 +212,8 @@ vcs_planes_kernel (const PlanesParams P, const VcsBatch frames)
 }
 
 // copy / halve planes with word-aligned rows on their own: one thread = one output word, the grid exactly the plane's words
-// (inside vcs_planes_kernel these modes ran on the byte kernel's grid with its register footprint: 10.6 us for the luma plane of
-// a 4K -> 1080p NV12 frame, 1 TB/s).  Same arithmetic as the vec4 branch above (video_orc_planar_chroma_*, avgub).
+// (inside vcs_planes_kernel these modes ran on the byte kernel's grid with its register footprint, far below the HBM
+// bandwidth).  Same arithmetic as the vec4 branch above (video_orc_planar_chroma_*, avgub).
 __global__ void __launch_bounds__ (256)
 vcs_planes_vec_kernel (const PlaneDev Q, const VcsBatch frames)
 {

@@ -1,4 +1,4 @@
-// gstreamer_b200/csrc/vcs_rgb420.cuh — packed RGB -> 4:2:0: matrix + chroma down-sampling + pack in one pass (product, sm_100a).
+// gstreamer_b200/csrc/vcs_rgb420.cuh — packed RGB -> 4:2:0: matrix + chroma down-sampling + pack in one pass (product, sm_90a).
 //
 // The encoder-feeding direction (BGRA / RGBA / ARGB / ABGR and their x forms -> NV12 / NV21 / I420 / YV12) at an unchanged
 // or shrinking size.  The reference has no table row for it and runs its chain (video-converter.c:2421-2560): unpack to

@@ -1,4 +1,4 @@
-// gstreamer_b200/csrc/vcs_yuy2_420.cuh — packed 4:2:2 -> planar 4:2:0 at an unchanged size (product, sm_100a).
+// gstreamer_b200/csrc/vcs_yuy2_420.cuh — packed 4:2:2 -> planar 4:2:0 at an unchanged size (product, sm_90a).
 //
 // The capture -> encoder rows of the reference's fast-path table (video-converter.c:8493-8507): YUY2 / UYVY -> I420 / YV12,
 // unchanged size, same colour matrix (range and chroma-site are not looked at, :8985-8997; a border rectangle or any other

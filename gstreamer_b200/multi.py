@@ -89,7 +89,7 @@ def _parse_cpulist(text):
 def bind_to_gpu_numa(local_gpu):
     """Pin this process (one pipeline per GPU) to the cores next to its GPU, BEFORE any staging memory is allocated or
     touched: one pipeline per GPU on a two-socket host otherwise pushes half of the H2D / D2H bytes across the socket
-    interconnect (round 1: per-GPU H2D fell from 49 to 22 GB/s at 8 pipelines).  Returns what it did, for the bench line."""
+    interconnect.  Returns what it did, for the bench line."""
     node, cpus = gpu_numa_cpus(local_gpu)
     if not cpus:
         return {"numa_node": node, "bound": False}

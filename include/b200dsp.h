@@ -1,4 +1,4 @@
-/* include/b200dsp.h — C-ABI of libb200dsp: the B200-native raw-frame DSP hot path.
+/* include/b200dsp.h — C-ABI of libb200dsp: the CUDA-native (H100, sm_90a) raw-frame DSP hot path.
  *
  * This is the drop-in boundary.  Every entry point is what a GStreamer element's
  * vmethod would call in place of the reference's CPU library call; the reference
@@ -189,8 +189,8 @@ typedef struct {
   int32_t smem_bytes;
   int32_t kernel_variant;        /* 0 = generic tiled, 1 = lanczos 2:1 specialised, 2 = light (copy / 2-tap axes), 3 = n-tap any ratio, 4 = YUV plane scaling,
                                   * 5 = chain + chroma down-sampling (4:2:0 -> the other 4:2:0 family; 2 launches),
-                                  * 6 = lanczos 2:1 with mma.sync FIRs (cross-check only: set_kernel_variant; measured slower),
-                                  * 7 = lanczos 2:1 with both FIR passes as tcgen05.mma.kind::i8 banded products, accumulators in TMEM
+                                  * 6 = lanczos 2:1 with mma.sync FIRs (cross-check only: set_kernel_variant; not timed on H100),
+                                  * 7 = lanczos 2:1 with both FIR passes as wgmma s8 x u8 banded products on the tensor cores
                                   *     (bit-exact; set_kernel_variant(7) or B200_L2_TC=1 - not the default, see DESIGN.md) */
   int32_t n_launches_per_convert;
 } b200_vcs_plan_info;

@@ -1,4 +1,4 @@
-/* refshim: <gst/gstcpuid.h> — report the SSE levels every x86-64 B200 host has, so the
+/* refshim: <gst/gstcpuid.h> — report the SSE levels every x86-64 host has, so the
  * reference picks the same SSE inner products its real x86 build uses
  * (gst-libs/gst/audio/audio-resampler-x86.h:29-70). */
 #ifndef B200_REFSHIM_CPUID_H

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the H100)")
     config.addinivalue_line("markers", "ref: needs oracle/_ref/libgstref.so (the compiled reference)")
 
 
@@ -27,7 +27,7 @@ def pytest_collection_modifyitems(config, items):
     have_gpu = _have_gpu() or os.environ.get("B200_REQUIRE_GPU") == "1"   # on the device box a missing GPU must fail loudly
     for item in items:
         if "gpu" in item.keywords and not have_gpu:
-            item.add_marker(pytest.mark.skip(reason="no CUDA device visible (gpu tests run on the B200 box)"))
+            item.add_marker(pytest.mark.skip(reason="no CUDA device visible (gpu tests run on the H100)"))
         if "ref" in item.keywords and not have_ref:
             item.add_marker(pytest.mark.skip(reason="oracle/_ref/libgstref.so not built"))
 

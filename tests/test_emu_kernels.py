@@ -108,7 +108,7 @@ SMALL = [(64, 48, 32, 24), (40, 30, 64, 48), (33, 17, 20, 31), (57, 35, 29, 35),
 @pytest.mark.parametrize("size", SMALL, ids=lambda s: "%dx%d-%dx%d" % s)
 def test_emulator_agrees_on_device_verified_paths(emu, size):
     """generic kernel (4:2:0 -> packed RGB), plane kernel (same family) and chain + chroma down-sampling (other family)
-    are bit-exact on a B200 (tests/test_vcs_gpu.py, _planes_gpu, _cross_gpu); the emulated build must say the same"""
+    are bit-exact on the GPU (tests/test_vcs_gpu.py, _planes_gpu, _cross_gpu); the emulated build must say the same"""
     iw, ih = size[:2]
     for fi, fo, method in [("NV12", "BGRA", 3), ("I420", "RGBA", 1), ("NV21", "xRGB", 0), ("NV12", "NV12", 1), ("I420", "YV12", 9),
                            ("NV12", "I420", 3), ("YV12", "NV21", 1), ("I420", "NV12", 0)]:
@@ -551,8 +551,7 @@ def test_audio_pipeline_many_tiles_per_cta(emu, monkeypatch, fmt):
 # ---- 5. the randomised three-way runs (tools/emu_fuzz*.py) keep working: a few seconds of each -------------------------
 @pytest.mark.parametrize("tool", ["emu_fuzz.py", "emu_fuzz_audio.py", "emu_fuzz_comp.py"])
 def test_random_run_tools(emu, tool):
-    """reference build (when present) vs oracle vs emulated kernels on random configurations; the long runs are recorded
-    in profiles/r01_race_check.txt"""
+    """reference build (when present) vs oracle vs emulated kernels on random configurations"""
     import subprocess
     import sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -1,5 +1,5 @@
-"""vcs_l2tc_kernel (kernel_variant 7): the exact-2:1 / 8-tap conversion with BOTH FIR passes on the 5th-generation
-tensor cores (tcgen05.mma.kind::i8, accumulators in TMEM, see gstreamer_b200/csrc/vcs_l2tc.cuh).  Bit-exact against
+"""vcs_l2tc_kernel (kernel_variant 7): the exact-2:1 / 8-tap conversion with BOTH FIR passes on the Hopper tensor
+cores (wgmma.mma_async s8 x u8, accumulators in registers, see gstreamer_b200/csrc/vcs_l2tc.cuh).  Bit-exact against
 the oracle on every shape class the tiling distinguishes: partial strips (width not a multiple of 128 output columns),
 partial row tiles (height not a multiple of 28 output rows), single-tile frames, frame-edge taps on all four sides,
 both chroma orders, every 8-tap method, batches."""
