@@ -20,18 +20,20 @@ GST_DEBUG_CATEGORY_STATIC (cuda_vcs_debug);
 #define GST_CAT_DEFAULT cuda_vcs_debug
 
 /* what b200_vcs_create accepts: every sink format to every src format - 4:2:0, packed RGB, packed 4:2:2 (capture) and planar
- * Y42B / Y444 in; packed RGB (scaling, byte order) or 4:2:0 (the encoder-feeding direction) out */
+ * Y42B / Y444 in; packed RGB (scaling, byte order), planar RGB (a network's CHW input) or 4:2:0 (the encoder-feeding
+ * direction) out */
 #define YUV420_FORMATS "NV12, NV21, I420, YV12"
 #define RGB_FORMATS "BGRA, RGBA, ARGB, ABGR, BGRx, RGBx, xRGB, xBGR"
 #define PACKED422_FORMATS "YUY2, UYVY, YVYU"
 #define PLANAR4XX_FORMATS "Y42B, Y444"
+#define PLANAR_RGB_FORMATS "RGBP, BGRP"
 #define CAPTURE_FORMATS PACKED422_FORMATS ", " PLANAR4XX_FORMATS
 #define SINK_FORMATS "{ " YUV420_FORMATS ", " RGB_FORMATS ", " CAPTURE_FORMATS " }"
 /* YUV outputs: the same family (NV12->NV12, NV21->NV21, I420/YV12 -> I420/YV12) scales plane by plane, the other
  * 4:2:0 pairs run the chain with chroma down-sampling; fixate_caps must carry the input colorimetry over
  * (transfer_colorimetry_from_input, gstvideoconvertscale.c:1335-1427) - b200_vcs_create refuses a YUV -> YUV
  * matrix change with B200_ERR_UNSUPPORTED */
-#define SRC_FORMATS "{ " RGB_FORMATS ", " YUV420_FORMATS " }"
+#define SRC_FORMATS "{ " RGB_FORMATS ", " PLANAR_RGB_FORMATS ", " YUV420_FORMATS " }"
 #define RAW_FIELDS(f) "format = (string) " f \
     ", width = (int) [ 1, 32767 ], height = (int) [ 1, 32767 ], framerate = (fraction) [ 0/1, max ]"
 /* device memory first (zero copy between CUDA elements), then plain system memory: in that case transform() hands the
@@ -198,7 +200,8 @@ vcs_query (GstBaseTransform * trans, GstPadDirection direction, GstQuery * query
   return GST_BASE_TRANSFORM_CLASS (gst_cuda_video_convert_scale_parent_class)->query (trans, direction, query);
 }
 
-/* 0: 4:2:0, 1: packed RGB, 2: planar 4:2:2 / 4:4:4, 3: packed 4:2:2, -1: not a fixed format name of ours */
+/* 0: 4:2:0, 1: packed RGB, 2: planar 4:2:2 / 4:4:4, 3: packed 4:2:2, 4: planar RGB, -1: not a fixed format name of ours
+ * (no name of one class is a substring of a name of another) */
 static gint
 vcs_format_class (const GstStructure * st)
 {
@@ -213,6 +216,8 @@ vcs_format_class (const GstStructure * st)
     return 2;
   if (strstr (PACKED422_FORMATS, f))
     return 3;
+  if (strstr (PLANAR_RGB_FORMATS, f))
+    return 4;
   return -1;
 }
 

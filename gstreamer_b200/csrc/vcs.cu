@@ -69,6 +69,8 @@ struct b200_vcs {
   int rgb420_pre = 0;             // 0: none, 1: vcs_rgb2ayuv_kernel, 2: vcs_yuy2_ayuv_kernel
   PlaneFastState rgb420_scaler;
   Yuy2Dev yuy2;                   // YUY2 / UYVY -> I420 / YV12 at an unchanged size (plan.yuy2_420)
+  DeintDev deint;                 // packed RGB -> RGBP / BGRP: the de-interleave (after planes' scaler into d_scratch if scaled)
+  bool deint_scaled = false;
   size_t in_bytes = 0, out_bytes = 0;
 };
 
@@ -180,6 +182,30 @@ int launch (b200_vcs * h, int n, const VcsBatch & batch, cudaStream_t stream)
 int launch_convert (b200_vcs * h, int n, const VcsBatch & batch, cudaStream_t stream)
 {
   const VcsPlan & p = h->plan;
+  if (p.planes_mode && p.rgbp_out) {
+    // packed RGB -> RGBP / BGRP: [the packed RGB scaler into the scratch image ->] de-interleave
+    DeintDev d = h->deint;
+    DeintBatch fin;
+    for (int i = 0; i < n; i++) { fin.src[i] = batch.in[i]; fin.out[i] = batch.out[i]; }
+    if (h->deint_scaled) {
+      const size_t frame = (size_t) d.sstride * d.h;
+      if (n > h->scratch_frames || frame != h->scratch_frame_bytes) {
+        B200_CUDA_TRY (cudaFree (h->d_scratch));                    // synchronises with launches still reading it
+        h->d_scratch = nullptr; h->scratch_frames = 0;
+        B200_CUDA_TRY (cudaMalloc ((void **) &h->d_scratch, frame * n));
+        h->scratch_frames = n; h->scratch_frame_bytes = frame;
+      }
+      VcsBatch mid;
+      bool aligned = true;
+      for (int i = 0; i < n; i++) {
+        mid.in[i] = batch.in[i]; mid.out[i] = h->d_scratch + frame * i; fin.src[i] = mid.out[i];
+        aligned = aligned && (((uintptr_t) batch.in[i]) & 7) == 0;
+      }
+      const int s = launch_planes (h->planes, mid, n, stream, aligned);
+      if (s != B200_OK) return s;
+    }
+    return launch_rgb_deinterleave (d, fin, n, stream);
+  }
   if (p.planes_mode) {
     bool aligned = true;                                            // the word-wide halve / copy path needs 8-byte aligned frames
     for (int i = 0; i < n; i++) aligned = aligned && ((((uintptr_t) batch.in[i]) | ((uintptr_t) batch.out[i])) & 7) == 0;
@@ -195,12 +221,12 @@ int launch_convert (b200_vcs * h, int n, const VcsBatch & batch, cudaStream_t st
     bool aligned = true;                                            // 16-byte cp.async of the luma rows
     for (int i = 0; i < n; i++) aligned = aligned && (((uintptr_t) batch.in[i]) & 15) == 0 && (((uintptr_t) batch.out[i]) & 3) == 0;
     if (aligned) return launch_l2tc (h->dev, h->tc, batch, n, stream);
-    if (p.lanczos2_ok && !p.planar) return launch_lanczos2 (h->dev, h->l2, batch, n, stream);
+    if (p.lanczos2_ok && !p.planar && !p.rgbp_out) return launch_lanczos2 (h->dev, h->l2, batch, n, stream);
   }
 #endif
   if (h->variant == 1 && p.lanczos2_ok && !p.yuv_out) {
-    if (h->l2v2.ready && h->l2.x4) return launch_lanczos2_v2 (h->dev, h->l2, h->l2v2, batch, n, stream);
-    if (!p.planar) return launch_lanczos2 (h->dev, h->l2, batch, n, stream);
+    if (h->l2v2.ready && h->l2.x4) return launch_lanczos2_v2 (h->dev, h->l2, h->l2v2, batch, n, stream, p.rgbp_out);
+    if (!p.planar && !p.rgbp_out) return launch_lanczos2 (h->dev, h->l2, batch, n, stream);
   }
   if (h->variant == 2 && p.light_ok && !p.yuv_out) {
     // 32-bit plane loads: the frame itself must be word aligned (device allocations always are)
@@ -300,7 +326,7 @@ int launch_convert (b200_vcs * h, int n, const VcsBatch & batch, cudaStream_t st
       const int s = launch_ntap (h->dev, p, h->ntap, mid, n, stream);
       if (s != B200_OK) return s;
     } else {
-      vcs_generic_kernel <<<grid, 256, p.smem_bytes, stream>>> (h->dev, mid);
+      vcs_generic_kernel<false> <<<grid, 256, p.smem_bytes, stream>>> (h->dev, mid);
       B200_CUDA_TRY (cudaGetLastError ());
     }
     if (p.extra_row) {
@@ -312,7 +338,7 @@ int launch_convert (b200_vcs * h, int n, const VcsBatch & batch, cudaStream_t st
       x.ih = 1; x.oh = 1; x.v.in_size = x.v.out_size = 1;
       x.off_out = (unsigned long long) p.out.height * x.stride_out;
       dim3 gx (grid.x, 1, n);
-      vcs_generic_kernel <<<gx, 256, p.smem_bytes, stream>>> (x, mid);
+      vcs_generic_kernel<false> <<<gx, 256, p.smem_bytes, stream>>> (x, mid);
       B200_CUDA_TRY (cudaGetLastError ());
     }
     const int cw = (p.out.width + 1) / 2, chh = (p.out.height + 1) / 2;
@@ -321,7 +347,8 @@ int launch_convert (b200_vcs * h, int n, const VcsBatch & batch, cudaStream_t st
     B200_CUDA_TRY (cudaGetLastError ());
     return B200_OK;
   }
-  vcs_generic_kernel <<<grid, 256, p.smem_bytes, stream>>> (h->dev, batch);
+  if (p.rgbp_out) vcs_generic_kernel<true> <<<grid, 256, p.smem_bytes, stream>>> (h->dev, batch);
+  else vcs_generic_kernel<false> <<<grid, 256, p.smem_bytes, stream>>> (h->dev, batch);
   B200_CUDA_TRY (cudaGetLastError ());
   return B200_OK;
 }
@@ -415,6 +442,12 @@ int b200_video_info_set_format (b200_video_info * info, int format, int width, i
       info->stride[0] = width * 4;      // video-info.c:890-894
       info->color_matrix = B200_COLOR_MATRIX_RGB; info->color_range = B200_COLOR_RANGE_0_255;
       return B200_OK;
+    case B200_VIDEO_FORMAT_RGBP: case B200_VIDEO_FORMAT_BGRP:        // video-info.c:1030-1041 (the Y444 case)
+      info->stride[0] = info->stride[1] = info->stride[2] = (width + 3) & ~3;
+      info->offset[1] = (uint64_t) info->stride[0] * height;
+      info->offset[2] = info->offset[1] * 2;
+      info->color_matrix = B200_COLOR_MATRIX_RGB; info->color_range = B200_COLOR_RANGE_0_255;
+      return B200_OK;
     case B200_VIDEO_FORMAT_I420_10LE: case B200_VIDEO_FORMAT_I420_12LE:       // video-info.c:1142-1156
     case B200_VIDEO_FORMAT_I422_10LE: case B200_VIDEO_FORMAT_I422_12LE: {     // :1157-1169
       const bool is420 = format == B200_VIDEO_FORMAT_I420_10LE || format == B200_VIDEO_FORMAT_I420_12LE;
@@ -460,6 +493,14 @@ size_t b200_video_info_size (const b200_video_info * info)
       return (size_t) info->offset[2] + (size_t) info->stride[2] * (((info->height + 1) & ~1) / 2);
     case B200_VIDEO_FORMAT_I422_10LE: case B200_VIDEO_FORMAT_I422_12LE:
       return (size_t) info->offset[2] + (size_t) info->stride[2] * ((info->height + 1) & ~1);
+    case B200_VIDEO_FORMAT_RGBP: case B200_VIDEO_FORMAT_BGRP: {       // three full planes in any order
+      size_t end = 0;
+      for (int k = 0; k < 3; k++) {
+        const size_t e = (size_t) info->offset[k] + (size_t) info->stride[k] * info->height;
+        if (e > end) end = e;
+      }
+      return end;
+    }
     default:
       return (size_t) info->offset[0] + (size_t) info->stride[0] * info->height;
   }
@@ -484,7 +525,11 @@ int b200_vcs_create (const b200_video_info * in, const b200_video_info * out,
     memset (&b, 0, sizeof (b));
     const bool rgb = f.format >= B200_VIDEO_FORMAT_RGBx && f.format <= B200_VIDEO_FORMAT_ABGR;
     const bool planar = f.format == B200_VIDEO_FORMAT_I420 || f.format == B200_VIDEO_FORMAT_YV12;
-    if (rgb) {
+    if (q.rgbp_out) {                                               // pack_RGBP of the border line: each plane its own byte
+      b.n_planes = 3;
+      for (int k = 0; k < 3; k++)
+        b.pl[k] = BorderPlane {f.offset[k], f.stride[k], f.width, f.height, 1, q.dest[0], q.dest[1], q.dest[2], q.dest[3], (unsigned) q.border_px[k]};
+    } else if (rgb) {
       b.n_planes = 1;
       b.pl[0] = BorderPlane {f.offset[0], f.stride[0], f.width, f.height, 4, q.dest[0], q.dest[1], q.dest[2], q.dest[3],
         (unsigned) q.border_px[0] | ((unsigned) q.border_px[1] << 8) | ((unsigned) q.border_px[2] << 16) | ((unsigned) q.border_px[3] << 24)};
@@ -514,7 +559,24 @@ int b200_vcs_create (const b200_video_info * in, const b200_video_info * out,
       if (device >= ndev) { delete h; return B200_ERR_INVALID_ARG; }
       DeviceGuard g (device);
       if (!g.ok) { delete h; return B200_ERR_CUDA; }
-      if ((st = prepare_planes (h->plan, &h->planes)) != B200_OK) { b200_vcs_destroy (h); return st; }
+      if (h->plan.rgbp_out) {
+        // packed RGB -> planar RGB: the scaler writes a scratch image of 4-byte pixels (16-byte aligned rows), the
+        // de-interleave reads it - or the input frame itself at an unchanged size
+        const VcsPlan & q = h->plan;
+        DeintDev & d = h->deint;
+        memset (&d, 0, sizeof (d));
+        d.w = q.out.width; d.h = q.out.height; d.sel = q.deint_sel;
+        for (int k = 0; k < 3; k++) { d.off[k] = q.out.offset[k]; d.stride[k] = q.out.stride[k]; }
+        h->deint_scaled = q.planes[0].mode == PM_SCALE;
+        if (h->deint_scaled) {
+          VcsPlan sp = q;
+          sp.out.offset[0] = 0; sp.out.stride[0] = (q.out.width * 4 + 15) & ~15;
+          d.soff = 0; d.sstride = sp.out.stride[0];
+          if ((st = prepare_planes (sp, &h->planes)) != B200_OK) { b200_vcs_destroy (h); return st; }
+        } else {
+          d.soff = q.in.offset[0]; d.sstride = q.in.stride[0];
+        }
+      } else if ((st = prepare_planes (h->plan, &h->planes)) != B200_OK) { b200_vcs_destroy (h); return st; }
     }
     *handle = h;
     return B200_OK;
@@ -529,14 +591,18 @@ int b200_vcs_create (const b200_video_info * in, const b200_video_info * out,
     h->l2_tables = build_lanczos2_tables (h->plan);
     h->l2v2_tables = build_lanczos2_v2_tables (h->plan, h->l2_tables);
     // planar (I420 / YV12) input exists in the second form of the kernel only
-    h->plan.lanczos2_ok = h->l2_tables.ok && (!h->plan.planar || (h->l2v2_tables.ok && !getenv ("B200_L2_V1") && !getenv ("B200_L2_X4")));
-    h->mma_tables = build_l2mma_tables (h->plan);
+    // planar RGB output: the second form only as well; the first form and the tensor forms (variants 6 / 7) decline it
+    const bool v2_only = h->plan.planar || h->plan.rgbp_out;
+    h->plan.lanczos2_ok = h->l2_tables.ok && (!v2_only || (h->l2v2_tables.ok && !getenv ("B200_L2_V1") && !getenv ("B200_L2_X4")));
+    if (!h->plan.rgbp_out) {
+      h->mma_tables = build_l2mma_tables (h->plan);
 #ifndef B200_CUDA_EMU
-    h->tc_tables = build_l2tc_tables (h->plan, h->l2_tables);
+      h->tc_tables = build_l2tc_tables (h->plan, h->l2_tables);
 #endif
+    }
   }
   const VcsPlan & p = h->plan;
-  if (!p.yuv_out && ((p.out.stride[0] & 3) || (p.out.offset[0] & 3))) { delete h; return B200_ERR_UNSUPPORTED; }
+  if (!p.yuv_out && !p.rgbp_out && ((p.out.stride[0] & 3) || (p.out.offset[0] & 3))) { delete h; return B200_ERR_UNSUPPORTED; }
   h->device = device;
   // the kernel this plan will run (also reported for host-only handles: caps negotiation dry-runs, CPU tests)
   h->variant = h->plan.lanczos2_ok ? 1 : (h->plan.light_ok ? 2 : (h->plan.ntap_ok ? 3 : 0));
@@ -599,6 +665,9 @@ int b200_vcs_create (const b200_video_info * in, const b200_video_info * out,
     d.sel = p.byte_sel[0] | (p.byte_sel[1] << 4) | (p.byte_sel[2] << 8) | (p.byte_sel[3] << 12);
     d.tile_w = p.tile_w; d.tile_h = p.tile_h; d.max_rows = p.max_rows; d.cols_pitch = p.cols_pitch;
     d.max_crows = p.max_crows;
+    for (int k = 0; k < 3; k++) {                                   // planar RGB output planes (store_planar_px)
+      d.off_pl[k] = p.rgbp_out ? p.out.offset[k] : 0; d.stride_pl[k] = p.rgbp_out ? p.out.stride[k] : 0;
+    }
     if ((st = upload_axis (p.h, &h->d_hoff, &h->d_hcoef, &h->d_hsum, &d.h)) != B200_OK ||
         (st = upload_axis (p.v, &h->d_voff, &h->d_vcoef, &h->d_vsum, &d.v)) != B200_OK ||
         (st = upload (&h->d_cmode, p.chroma_mode.data (), p.chroma_mode.size ())) != B200_OK) {
@@ -606,7 +675,7 @@ int b200_vcs_create (const b200_video_info * in, const b200_video_info * out,
       return st;
     }
     d.chroma_mode = h->d_cmode;
-    if ((st = allow_max_dyn_smem (vcs_generic_kernel)) != B200_OK) { b200_vcs_destroy (h); return st; }
+    if ((st = allow_max_dyn_smem (p.rgbp_out ? vcs_generic_kernel<true> : vcs_generic_kernel<false>)) != B200_OK) { b200_vcs_destroy (h); return st; }
     if (h->mma_tables.ok) {
       st = prepare_l2mma (h->mma_tables, &h->mma);
       if (st != B200_OK) { b200_vcs_destroy (h); return st; }
@@ -760,7 +829,7 @@ int b200_vcs_get_plan_info (const b200_vcs * h, b200_vcs_plan_info * info)
   for (int i = 0; i < 5; i++) info->p[i] = p.p[i];
   info->tile_w = p.tile_w; info->tile_h = p.tile_h; info->smem_bytes = p.smem_bytes;
   info->kernel_variant = p.yuv_out ? 5 : p.planes_mode ? 4 : h->variant == 7 ? 7 : (h->variant == 6 && h->mma.ready) ? 6 : (h->variant == 1 && p.lanczos2_ok) ? 1 : (h->variant == 2 && p.light_ok) ? 2 : (h->variant == 3 && p.ntap_ok) ? 3 : 0;
-  info->n_launches_per_convert = (p.yuy2_420 ? 1 : h->rgb420_ok ? (1 + (h->rgb420_pre ? 1 : 0) + (h->rgb420_scaled ? 1 : 0)) : p.yuv_out ? (p.extra_row ? 3 : 2) : 1) + (p.has_dest && p.fill_border ? 1 : 0);
+  info->n_launches_per_convert = (p.rgbp_out && p.planes_mode ? (p.planes[0].mode == PM_SCALE ? 2 : 1) : p.yuy2_420 ? 1 : h->rgb420_ok ? (1 + (h->rgb420_pre ? 1 : 0) + (h->rgb420_scaled ? 1 : 0)) : p.yuv_out ? (p.extra_row ? 3 : 2) : 1) + (p.has_dest && p.fill_border ? 1 : 0);
   return B200_OK;
 }
 
@@ -817,6 +886,7 @@ const char *b200_vcs_kernel_name (const b200_vcs * h)
 {
   if (!h) return "";
   const VcsPlan & p = h->plan;
+  if (p.planes_mode && p.rgbp_out) return "vcs_rgb_deinterleave_kernel";
   if (p.planes_mode) {
     for (int i = 0; i < p.n_planes; i++) if (h->planes.fast[i].ok) return h->planes.fast[i].vfirst ? "vcs_planes_fast_vfirst_kernel" : "vcs_planes_fast_kernel";
     return "vcs_planes_kernel";

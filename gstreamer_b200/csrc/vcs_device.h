@@ -41,6 +41,9 @@ struct VcsDev {
   AxisDev h, v;
   const uint8_t *chroma_mode;    // [ih]
   int tile_w, tile_h, max_rows, cols_pitch, max_crows;
+  // planar RGB output (the kernels' planar store form): byte k of the packed pixel goes to plane k
+  unsigned long long off_pl[3];
+  int stride_pl[3];
 };
 
 struct VcsBatch {

@@ -108,6 +108,15 @@ __device__ __forceinline__ unsigned pack_px (int a, int r, int g, int b, unsigne
   return __byte_perm (argb, 0, sel);
 }
 
+// planar RGB store form (RGBP / BGRP): bytes 0..2 of the packed pixel `px` (the plan's byte selector is that of RGBx /
+// BGRx) go to planes 0..2.  A lane owns one output column, so a warp's byte stores to a plane row are consecutive.
+__device__ __forceinline__ void store_planar_px (const VcsDev & P, uint8_t *out, int ox, int oy, unsigned px)
+{
+  out[P.off_pl[0] + (size_t) oy * P.stride_pl[0] + ox] = (uint8_t) px;
+  out[P.off_pl[1] + (size_t) oy * P.stride_pl[1] + ox] = (uint8_t) (px >> 8);
+  out[P.off_pl[2] + (size_t) oy * P.stride_pl[2] + ox] = (uint8_t) (px >> 16);
+}
+
 // ------------------------------------------------------------------------------------------
 // Generic fused kernel: one CTA = one output tile of one frame.
 //   A1  h-upsampled chroma rows of the tile's input region  -> smem
@@ -115,7 +124,9 @@ __device__ __forceinline__ unsigned pack_px (int a, int r, int g, int b, unsigne
 //   B   first separable pass                                -> smem planes T[3]
 //   C   second pass + matrix + alpha + pack                 -> global (coalesced 4 B / thread)
 // Handles every scale method / ratio / order the plan builder can emit.
+// PLOUT: planar RGB output (store_planar_px) instead of one 4-byte word per pixel.
 // ------------------------------------------------------------------------------------------
+template <bool PLOUT = false>
 __global__ void __launch_bounds__ (256)
 vcs_generic_kernel (const VcsDev P, const VcsBatch frames)
 {
@@ -278,6 +289,10 @@ vcs_generic_kernel (const VcsDev P, const VcsBatch frames)
     int a = 255;
     if (P.h_first) { a = alpha_pass (a, P.h, ox); a = alpha_pass (a, P.v, oy); }
     else { a = alpha_pass (a, P.v, oy); a = alpha_pass (a, P.h, ox); }
+    if (PLOUT) {
+      store_planar_px (P, out, ox, oy, pack_px (a, r, g, b, P.sel));
+      continue;
+    }
     unsigned *dst = (unsigned *) (out + P.off_out + (size_t) oy * P.stride_out) + ox;
     *dst = pack_px (a, r, g, b, P.sel);
   }

@@ -66,9 +66,10 @@ __device__ __forceinline__ unsigned pack_sat_s16x2 (int a, int b)     // { sat_s
 // PF: 1 the next H item's loads are issued before this item's arithmetic, 2 only its chroma rows, 0 neither.
 // PLANAR: I420 / YV12 input - a chroma row is one 32-bit word from each of the U and V planes (already de-interleaved).
 // YUVOUT: 4:2:0 output through the chain (VcsDev::yuv_out): no matrix stage, {255, Y, U, V} pixels for vcs_down420_kernel.
+// PLOUT: planar RGB output (RGBP / BGRP): the packed pixel's bytes 0..2 go to three planes (store_planar_px).
 // TH x NT: output rows per tile and threads per CTA (60 x 256 at 4 CTAs per SM, or 124 x 512 at 2: 256 of 254 filtered lines used
 // instead of 128 of 126).
-template <int MINB, int SEL, int PF, int TH = 60, int NT = L2_THREADS, bool PLANAR = false, bool YUVOUT = false>
+template <int MINB, int SEL, int PF, int TH = 60, int NT = L2_THREADS, bool PLANAR = false, bool YUVOUT = false, bool PLOUT = false>
 __global__ void __launch_bounds__ (NT, MINB)
 vcs_lanczos2_v2_kernel (const VcsDev P, const Lanczos2Dev L, const Lanczos2V2Dev K, const VcsBatch frames)
 {
@@ -347,7 +348,8 @@ vcs_lanczos2_v2_kernel (const VcsDev P, const Lanczos2Dev L, const Lanczos2V2Dev
           } else {
             px = __byte_perm (pack_sat2 (r, 255, pack_sat2 (b, gg, 0u)), 0, P.sel);
           }
-          *(unsigned *) (rowp[i] + 128 * k) = px;
+          if (PLOUT) store_planar_px (P, out, ox, oy + i, px);
+          else *(unsigned *) (rowp[i] + 128 * k) = px;
         }
       }
     }
@@ -433,11 +435,11 @@ inline int prepare_lanczos2_v2 (const Lanczos2V2Tables & t, Lanczos2V2State * st
   return B200_OK;
 }
 
-template <int SEL, int PF, int MINB = 4, int TH = 60, int NT = L2_THREADS, bool PLANAR = false, bool YUVOUT = false>
+template <int SEL, int PF, int MINB = 4, int TH = 60, int NT = L2_THREADS, bool PLANAR = false, bool YUVOUT = false, bool PLOUT = false>
 inline int launch_lanczos2_v2_sel (const VcsDev & d, const Lanczos2State & st, const Lanczos2V2State & v2, const VcsBatch & batch,
     int n, cudaStream_t stream)
 {
-  auto kern = vcs_lanczos2_v2_kernel<MINB, SEL, PF, TH, NT, PLANAR, YUVOUT>;
+  auto kern = vcs_lanczos2_v2_kernel<MINB, SEL, PF, TH, NT, PLANAR, YUVOUT, PLOUT>;
   static bool attr_done[16] = {false};
   int dev = 0; cudaGetDevice (&dev);
   if (!attr_done[dev & 15]) {
@@ -451,8 +453,16 @@ inline int launch_lanczos2_v2_sel (const VcsDev & d, const Lanczos2State & st, c
 }
 
 inline int launch_lanczos2_v2 (const VcsDev & d, const Lanczos2State & st, const Lanczos2V2State & v2, const VcsBatch & batch, int n,
-    cudaStream_t stream)
+    cudaStream_t stream, bool planar_out = false)
 {
+  if (planar_out) {                               // RGBP (sel of RGBx) / BGRP (sel of BGRx)
+    const bool bgr = d.sel == 0x0123u;
+    if (d.planar)
+      return bgr ? launch_lanczos2_v2_sel<0x0123, 0, 4, 60, L2_THREADS, true, false, true> (d, st, v2, batch, n, stream)
+                 : launch_lanczos2_v2_sel<0x0321, 0, 4, 60, L2_THREADS, true, false, true> (d, st, v2, batch, n, stream);
+    return bgr ? launch_lanczos2_v2_sel<0x0123, 0, 4, 60, L2_THREADS, false, false, true> (d, st, v2, batch, n, stream)
+               : launch_lanczos2_v2_sel<0x0321, 0, 4, 60, L2_THREADS, false, false, true> (d, st, v2, batch, n, stream);
+  }
   if (d.yuv_out)                                  // the cross-family chain's first launch: scaled {255, Y, U, V} pixels, no matrix
     return d.planar ? launch_lanczos2_v2_sel<-1, 0, 4, 60, L2_THREADS, true, true> (d, st, v2, batch, n, stream)
                     : launch_lanczos2_v2_sel<-1, 0, 4, 60, L2_THREADS, false, true> (d, st, v2, batch, n, stream);

@@ -393,7 +393,8 @@ __device__ __forceinline__ void vcs_unpack_fast_cs (const VcsDev & P, const uint
   else vcs_unpack_fast_cs_impl<MFIRST, LAYOUT, false> (P, in, cxa, cx1, ry0, R, S, pitch, plane_words);
 }
 
-template <int HM, int VM, bool MFIRST, bool COSITED>
+// PLOUT: planar RGB output (store_planar_px) instead of one 4-byte word per pixel
+template <int HM, int VM, bool MFIRST, bool COSITED, bool PLOUT = false>
 __global__ void __launch_bounds__ (LIGHT_THREADS, 4)
 vcs_light_kernel (const VcsDev P, const LightDev G, const VcsBatch frames)
 {
@@ -449,10 +450,11 @@ vcs_light_kernel (const VcsDev P, const LightDev G, const VcsBatch frames)
       // instructions per output pixel of which 30 were the loop's own.)
       const int half = (((th + 1) >> 1) + 1) & ~1, t0 = rph * half, t1 = min (th, t0 + half);
       uint8_t *dst = out + P.off_out + (size_t) (oy0 + t0) * P.stride_out + (size_t) (ox0 + tx) * 4u;
-      auto finish = [&] (unsigned d, uint8_t *q) {
+      auto finish = [&] (unsigned d, uint8_t *q, int ty) {
         if (!MFIRST) d = light_matrix (d, P);
         else d |= 0x000000ffu;                                    // alpha passes every 2-tap/copy stage as 255
-        *(unsigned *) q = __byte_perm (d, 0, P.sel);
+        if (PLOUT) store_planar_px (P, out, ox0 + tx, oy0 + ty, __byte_perm (d, 0, P.sel));
+        else *(unsigned *) q = __byte_perm (d, 0, P.sel);
       };
       for (int ty = t0; ty < t1; ty += 2, dst += 2 * (size_t) P.stride_out) {
         const bool two = ty + 1 < t1;
@@ -476,8 +478,8 @@ vcs_light_kernel (const VcsDev P, const LightDev G, const VcsBatch frames)
           d0 = hrow (a0);
           d1 = a1 == a0 ? d0 : hrow (a1);
         }
-        finish (d0, dst);
-        if (two) finish (d1, dst + P.stride_out);
+        finish (d0, dst, ty);
+        if (two) finish (d1, dst + P.stride_out, ty + 1);
       }
     }
   } else {
@@ -506,7 +508,8 @@ vcs_light_kernel (const VcsDev P, const LightDev G, const VcsBatch frames)
         if (HM == 2) d = light_lerp (d, t[1], 256u - f, f, 0u);
         if (!MFIRST) d = light_matrix (d, P);
         else d |= 0x000000ffu;
-        *(unsigned *) dst = __byte_perm (d, 0, P.sel);
+        if (PLOUT) store_planar_px (P, out, ox0 + tx, oy0 + ty, __byte_perm (d, 0, P.sel));
+        else *(unsigned *) dst = __byte_perm (d, 0, P.sel);
       }
     }
   }
@@ -518,6 +521,10 @@ inline light_kernel_fn light_kernel_for (const VcsPlan & p)
 {
 #define LIGHT_PICK(HM, VM)                                                                            \
   if (p.h.mode == HM && p.v.mode == VM) {                                                             \
+    if (p.rgbp_out) {                                                                                 \
+      if (p.matrix_first) return p.h_cosited ? vcs_light_kernel<HM, VM, true, true, true> : vcs_light_kernel<HM, VM, true, false, true>;   \
+      return p.h_cosited ? vcs_light_kernel<HM, VM, false, true, true> : vcs_light_kernel<HM, VM, false, false, true>;                     \
+    }                                                                                                 \
     if (p.matrix_first) return p.h_cosited ? vcs_light_kernel<HM, VM, true, true> : vcs_light_kernel<HM, VM, true, false>;   \
     return p.h_cosited ? vcs_light_kernel<HM, VM, false, true> : vcs_light_kernel<HM, VM, false, false>;                     \
   }

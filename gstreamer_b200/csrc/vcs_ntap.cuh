@@ -39,7 +39,8 @@ struct NtapDev {
 constexpr int NTAP_THREADS = 256;
 
 // NTW > 0: both n-tap axes use exactly NTW packed tap words (straight-line FIRs); NTW == 0: run-time loops
-template <int HM, int VM, bool MFIRST, bool COSITED, int NTW>
+// PLOUT: planar RGB output (store_planar_px) instead of one 4-byte word per pixel
+template <int HM, int VM, bool MFIRST, bool COSITED, int NTW, bool PLOUT = false>
 __global__ void __launch_bounds__ (NTAP_THREADS, 2)
 vcs_ntap_kernel (const VcsDev P, const NtapDev G, const VcsBatch frames)
 {
@@ -189,7 +190,8 @@ vcs_ntap_kernel (const VcsDev P, const NtapDev G, const VcsBatch frames)
         argb = light_matrix (pack_sat2 (c1, c0, pack_sat2 (0, c2, 0u)), P);
         if (!G.alpha_opaque) argb = (argb & 0xffffff00u) | (unsigned) al;
       }
-      *(unsigned *) dst = __byte_perm (argb, 0, P.sel);
+      if (PLOUT) store_planar_px (P, out, ox, oy0 + ty, __byte_perm (argb, 0, P.sel));
+      else *(unsigned *) dst = __byte_perm (argb, 0, P.sel);
     }
   }
 }
@@ -201,7 +203,7 @@ vcs_ntap_kernel (const VcsDev P, const NtapDev G, const VcsBatch frames)
 //      32-bit IMAD — the low lane is exact modulo 2^16, the high lane is off by the low lane's borrow, which
 //      bit 15 of the low lane gives back (|sums| < 2^15 is an eligibility condition).  One word = 4 columns.
 //  C'  horizontal FIR per output pixel with funnel shift + IDP.4A on the v-scaled rows, matrix, pack.
-template <int HM, int VM, bool MFIRST, bool COSITED>
+template <int HM, int VM, bool MFIRST, bool COSITED, bool PLOUT = false>
 __global__ void __launch_bounds__ (NTAP_THREADS, 2)
 vcs_ntap_vfirst_kernel (const VcsDev P, const NtapDev G, const VcsBatch frames)
 {
@@ -314,18 +316,25 @@ vcs_ntap_vfirst_kernel (const VcsDev P, const NtapDev G, const VcsBatch frames)
         argb = light_matrix (pack_sat2 (c[1], c[0], pack_sat2 (0, c[2], 0u)), P);
         if (!G.alpha_opaque) argb = (argb & 0xffffff00u) | (unsigned) al;
       }
-      *(unsigned *) dst = __byte_perm (argb, 0, P.sel);
+      if (PLOUT) store_planar_px (P, out, ox, oy0 + ty, __byte_perm (argb, 0, P.sel));
+      else *(unsigned *) dst = __byte_perm (argb, 0, P.sel);
     }
   }
 }
 
 typedef void (*ntap_kernel_fn) (const VcsDev, const NtapDev, const VcsBatch);
 
+template <int HM, int VM, int NTW, bool PLOUT>
+inline ntap_kernel_fn ntap_kernel_pick_out (const VcsPlan & p)
+{
+  if (p.matrix_first) return p.h_cosited ? vcs_ntap_kernel<HM, VM, true, true, NTW, PLOUT> : vcs_ntap_kernel<HM, VM, true, false, NTW, PLOUT>;
+  return p.h_cosited ? vcs_ntap_kernel<HM, VM, false, true, NTW, PLOUT> : vcs_ntap_kernel<HM, VM, false, false, NTW, PLOUT>;
+}
+
 template <int HM, int VM, int NTW>
 inline ntap_kernel_fn ntap_kernel_pick (const VcsPlan & p)
 {
-  if (p.matrix_first) return p.h_cosited ? vcs_ntap_kernel<HM, VM, true, true, NTW> : vcs_ntap_kernel<HM, VM, true, false, NTW>;
-  return p.h_cosited ? vcs_ntap_kernel<HM, VM, false, true, NTW> : vcs_ntap_kernel<HM, VM, false, false, NTW>;
+  return p.rgbp_out ? ntap_kernel_pick_out<HM, VM, NTW, true> (p) : ntap_kernel_pick_out<HM, VM, NTW, false> (p);
 }
 
 template <int HM, int VM>
@@ -341,11 +350,17 @@ inline ntap_kernel_fn ntap_kernel_pick_ntw (const VcsPlan & p)
   }
 }
 
+template <int HM, int VM, bool PLOUT>
+inline ntap_kernel_fn ntap_vfirst_pick_out (const VcsPlan & p)
+{
+  if (p.matrix_first) return p.h_cosited ? vcs_ntap_vfirst_kernel<HM, VM, true, true, PLOUT> : vcs_ntap_vfirst_kernel<HM, VM, true, false, PLOUT>;
+  return p.h_cosited ? vcs_ntap_vfirst_kernel<HM, VM, false, true, PLOUT> : vcs_ntap_vfirst_kernel<HM, VM, false, false, PLOUT>;
+}
+
 template <int HM, int VM>
 inline ntap_kernel_fn ntap_vfirst_pick (const VcsPlan & p)
 {
-  if (p.matrix_first) return p.h_cosited ? vcs_ntap_vfirst_kernel<HM, VM, true, true> : vcs_ntap_vfirst_kernel<HM, VM, true, false>;
-  return p.h_cosited ? vcs_ntap_vfirst_kernel<HM, VM, false, true> : vcs_ntap_vfirst_kernel<HM, VM, false, false>;
+  return p.rgbp_out ? ntap_vfirst_pick_out<HM, VM, true> (p) : ntap_vfirst_pick_out<HM, VM, false> (p);
 }
 
 inline ntap_kernel_fn ntap_kernel_for (const VcsPlan & p)

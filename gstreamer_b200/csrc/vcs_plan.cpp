@@ -655,10 +655,51 @@ static int build_rgb_same_plan (VcsPlan * p)
   return B200_OK;
 }
 
+static bool is_rgbp (int format)
+{
+  return format == B200_VIDEO_FORMAT_RGBP || format == B200_VIDEO_FORMAT_BGRP;
+}
+
+// every plane of a planar RGB output holds at least a row of the frame
+static bool rgbp_strides_ok (const b200_video_info & o)
+{
+  return o.stride[0] >= o.width && o.stride[1] >= o.width && o.stride[2] >= o.width;
+}
+
+// packed RGB -> RGBP / BGRP: the reference's chain without a matrix (both sides name the RGB matrix) - unpack to ARGB,
+// the scalers in chain_scale's pass order (like another packed RGB order, build_rgb_same_plan), pack_RGBP / pack_BGRP
+// (video-format.c:7496-7536: R, G, B bytes, alpha dropped).  Every byte is an independent channel, so the 4-byte
+// pixels are scaled in the input's own byte order and the de-interleave picks the components.
+static int build_rgb_rgbp_plan (VcsPlan * p)
+{
+  const b200_video_info *in = &p->in, *out = &p->out;
+  const int iw = in->width, ih = in->height, ow = out->width, oh = out->height;
+  if (in->stride[0] < iw * 4 || !rgbp_strides_ok (*out)) return B200_ERR_INVALID_ARG;
+  int pi[4];
+  rgb_component_bytes (in->format, pi);
+  const bool bgr = out->format == B200_VIDEO_FORMAT_BGRP;
+  p->rgbp_out = true;
+  p->deint_sel = (unsigned) pi[bgr ? 3 : 1] | (unsigned) pi[2] << 4 | (unsigned) pi[bgr ? 1 : 3] << 8;
+  const FilterSpec f = filter_from_method (p->cfg);
+  p->planes_mode = true;
+  p->n_planes = 1;
+  PlanePlan & q = p->planes[0];
+  q = PlanePlan ();
+  q.src_plane = 0; q.iw = iw; q.ih = ih; q.ow = ow; q.oh = oh; q.ne = 4;
+  if (iw == ow && ih == oh) { q.mode = PM_COPY; return B200_OK; }   // the de-interleave reads the frame itself
+  q.mode = PM_SCALE;
+  q.have_h = iw != ow; q.have_v = ih != oh;
+  if (q.have_h) scaled_axis (&q.h, f, iw, ow, true, true); else identity_axis (&q.h, iw);
+  if (q.have_v) scaled_axis (&q.v, f, ih, oh, false); else identity_axis (&q.v, ih);
+  q.h_first = (int64_t) ow * ih <= (int64_t) iw * oh;
+  return B200_OK;
+}
+
 static int build_rgb_in_plan (VcsPlan * p)
 {
   const b200_video_info *in = &p->in, *out = &p->out;
   if (out->format >= B200_VIDEO_FORMAT_RGBx && out->format <= B200_VIDEO_FORMAT_ABGR) return build_rgb_same_plan (p);
+  if (is_rgbp (out->format)) return build_rgb_rgbp_plan (p);
   const bool out_pl = out->format == B200_VIDEO_FORMAT_I420 || out->format == B200_VIDEO_FORMAT_YV12;
   const bool out_semi = out->format == B200_VIDEO_FORMAT_NV12 || out->format == B200_VIDEO_FORMAT_NV21;
   if (!out_pl && !out_semi) return B200_ERR_UNSUPPORTED;
@@ -716,13 +757,14 @@ static int build_inner_plan (const b200_video_info * in, const b200_video_info *
 static int border_colour (VcsPlan * p, const b200_video_info & fo, uint32_t argb_word)
 {
   const int a = argb_word >> 24, r = (argb_word >> 16) & 0xff, g = (argb_word >> 8) & 0xff, b = argb_word & 0xff;
-  const bool rgb = fo.format >= B200_VIDEO_FORMAT_RGBx && fo.format <= B200_VIDEO_FORMAT_ABGR;
+  const bool rgb = (fo.format >= B200_VIDEO_FORMAT_RGBx && fo.format <= B200_VIDEO_FORMAT_ABGR) || is_rgbp (fo.format);
   if (rgb) {
+    // RGBP / BGRP: border_px[k] is the byte of plane k (pack_RGBP / pack_BGRP of the border line)
     const uint8_t comp[4] = {(uint8_t) a, (uint8_t) r, (uint8_t) g, (uint8_t) b};
     uint8_t sel[4];
     switch (fo.format) {
-      case B200_VIDEO_FORMAT_BGRA: case B200_VIDEO_FORMAT_BGRx: { uint8_t s_[4] = {3, 2, 1, 0}; memcpy (sel, s_, 4); break; }
-      case B200_VIDEO_FORMAT_RGBA: case B200_VIDEO_FORMAT_RGBx: { uint8_t s_[4] = {1, 2, 3, 0}; memcpy (sel, s_, 4); break; }
+      case B200_VIDEO_FORMAT_BGRA: case B200_VIDEO_FORMAT_BGRx: case B200_VIDEO_FORMAT_BGRP: { uint8_t s_[4] = {3, 2, 1, 0}; memcpy (sel, s_, 4); break; }
+      case B200_VIDEO_FORMAT_RGBA: case B200_VIDEO_FORMAT_RGBx: case B200_VIDEO_FORMAT_RGBP: { uint8_t s_[4] = {1, 2, 3, 0}; memcpy (sel, s_, 4); break; }
       case B200_VIDEO_FORMAT_ABGR: case B200_VIDEO_FORMAT_xBGR: { uint8_t s_[4] = {0, 3, 2, 1}; memcpy (sel, s_, 4); break; }
       default: { uint8_t s_[4] = {0, 1, 2, 3}; memcpy (sel, s_, 4); break; }
     }
@@ -785,9 +827,12 @@ int build_vcs_plan (const b200_video_info * in, const b200_video_info * out,
   if (dw > out->width - dx) dw = out->width - dx;
   if (dh > out->height - dy) dh = out->height - dy;
   if (dw < 1 || dh < 1) return B200_ERR_INVALID_ARG;               // an empty rectangle: degenerate in the reference too
+  if (is_rgbp (out->format) && !rgbp_strides_ok (*out)) return B200_ERR_INVALID_ARG;
   b200_video_info inner = *out;
   inner.width = dw; inner.height = dh;
-  if (!yuv) inner.offset[0] += (uint64_t) dy * out->stride[0] + (uint64_t) dx * 4;
+  if (is_rgbp (out->format)) {                                     // no sub-sampling: every plane at (dx, dy)
+    for (int k = 0; k < 3; k++) inner.offset[k] += (uint64_t) dy * out->stride[k] + (uint64_t) dx;
+  } else if (!yuv) inner.offset[0] += (uint64_t) dy * out->stride[0] + (uint64_t) dx * 4;
   else {
     inner.offset[0] += (uint64_t) dy * out->stride[0] + (uint64_t) dx;
     if (planar) {
@@ -838,8 +883,8 @@ static int build_inner_plan (const b200_video_info * in, const b200_video_info *
     // Packed 4:2:2 (YUY2 / UYVY / YVYU) also converts to 4:2:0 (capture -> encoder): the chain closed by chroma
     // down-sampling, or the table rows YUY2 / UYVY -> I420 / YV12 at an unchanged size (yuy2_420 below).  Planar
     // 4:2:2 / 4:4:4 -> planar 4:2:0 are plane-scaling table rows, -> semi-planar 4:2:0 the chain again.
-    const bool out_rgb = out->format >= B200_VIDEO_FORMAT_RGBx && out->format <= B200_VIDEO_FORMAT_ABGR;
-    const bool out_420 = out->format == B200_VIDEO_FORMAT_I420 || out->format == B200_VIDEO_FORMAT_YV12 ||
+    const bool out_rgb = (out->format >= B200_VIDEO_FORMAT_RGBx && out->format <= B200_VIDEO_FORMAT_ABGR) || is_rgbp (out->format);
+    const bool out_420 =out->format == B200_VIDEO_FORMAT_I420 || out->format == B200_VIDEO_FORMAT_YV12 ||
         out->format == B200_VIDEO_FORMAT_NV12 || out->format == B200_VIDEO_FORMAT_NV21;
     const bool in_packed = in->format == B200_VIDEO_FORMAT_YUY2 || in->format == B200_VIDEO_FORMAT_UYVY || in->format == B200_VIDEO_FORMAT_YVYU;
     const bool out_pl420 = out->format == B200_VIDEO_FORMAT_I420 || out->format == B200_VIDEO_FORMAT_YV12;
@@ -926,14 +971,17 @@ static int build_inner_plan (const b200_video_info * in, const b200_video_info *
     { uint8_t s[4] = {0, 1, 2, 3}; memcpy (p->byte_sel, s, 4); }   // scratch pixels stay A,Y,U,V
   } else
   switch (out->format) {                // (A,R,G,B) component placed at each output byte
-    case B200_VIDEO_FORMAT_BGRA: case B200_VIDEO_FORMAT_BGRx: { uint8_t s[4] = {3, 2, 1, 0}; memcpy (p->byte_sel, s, 4); break; }
-    case B200_VIDEO_FORMAT_RGBA: case B200_VIDEO_FORMAT_RGBx: { uint8_t s[4] = {1, 2, 3, 0}; memcpy (p->byte_sel, s, 4); break; }
+    // RGBP / BGRP: the byte order of RGBx / BGRx puts plane k's component in byte k of the packed pixel
+    case B200_VIDEO_FORMAT_BGRA: case B200_VIDEO_FORMAT_BGRx: case B200_VIDEO_FORMAT_BGRP: { uint8_t s[4] = {3, 2, 1, 0}; memcpy (p->byte_sel, s, 4); break; }
+    case B200_VIDEO_FORMAT_RGBA: case B200_VIDEO_FORMAT_RGBx: case B200_VIDEO_FORMAT_RGBP: { uint8_t s[4] = {1, 2, 3, 0}; memcpy (p->byte_sel, s, 4); break; }
     case B200_VIDEO_FORMAT_ABGR: case B200_VIDEO_FORMAT_xBGR: { uint8_t s[4] = {0, 3, 2, 1}; memcpy (p->byte_sel, s, 4); break; }
     case B200_VIDEO_FORMAT_ARGB: case B200_VIDEO_FORMAT_xRGB: { uint8_t s[4] = {0, 1, 2, 3}; memcpy (p->byte_sel, s, 4); break; }
     default: return B200_ERR_UNSUPPORTED;
   }
+  p->rgbp_out = is_rgbp (out->format);
+  if (p->rgbp_out && !rgbp_strides_ok (*out)) return B200_ERR_INVALID_ARG;
   p->planar = in->format == B200_VIDEO_FORMAT_I420 || in->format == B200_VIDEO_FORMAT_YV12;
-  const int min_out_stride = p->yuv_out ? out->width : out->width * 4;
+  const int min_out_stride = (p->yuv_out || p->rgbp_out) ? out->width : out->width * 4;
   if (p->in_422_444) {
     if (out->stride[0] < min_out_stride) return B200_ERR_INVALID_ARG;
   } else if (p->planar) {
@@ -965,8 +1013,9 @@ static int build_inner_plan (const b200_video_info * in, const b200_video_info *
   chroma_pairing (p);
   // unchanged size, planar 4:2:0 in, packed RGB out: the reference never builds the chain, its fast path
   // (convert_I420_BGRA / _ARGB / _pack_ARGB, video-converter.c:6772-6988, table :8766-8800) feeds each
-  // chroma sample to its 2x2 pixels unfiltered
-  p->chroma_nearest = !p->yuv_out && p->planar && iw == ow && ih == oh;
+  // chroma sample to its 2x2 pixels unfiltered.  Planar RGB outputs have no such table row (video-converter.c:8766-8806
+  // lists packed outputs only): they run the chain, chroma up-sampling included.
+  p->chroma_nearest = !p->yuv_out && !p->rgbp_out && p->planar && iw == ow && ih == oh;
   if (p->chroma_nearest) {
     p->v_pairs = false;
     std::fill (p->chroma_mode.begin (), p->chroma_mode.end (), 0);

@@ -94,6 +94,14 @@ struct VcsPlan {
   uint8_t border_px[4] = {0, 0, 0, 0};   // packed RGB outputs: the border pixel in memory order
   int border_yuv[3] = {16, 128, 128};    // 4:2:0 outputs
 
+  // planar RGB output (RGBP / BGRP).  YUV inputs: the packed RGB plan with the byte selector of RGBx / BGRx, so that
+  // byte k of each packed pixel is the component of plane k; the kernels' planar store form writes it to
+  // out.offset[k] + y * out.stride[k] + x.  Packed RGB inputs: planes[0] scales the 4-byte pixels (input byte order)
+  // into a scratch image when the size changes, then a de-interleave launch writes plane k from source byte
+  // (deint_sel >> 4k) & 3.
+  bool rgbp_out = false;
+  unsigned deint_sel = 0;
+
   // specialised 2:1 lanczos kernel eligibility
   bool lanczos2_ok = false;
 

@@ -1,6 +1,6 @@
 // gstreamer_b200/csrc/vcs_planes.cuh — YUV -> same YUV family (NV12->NV12, NV21->NV21, I420/YV12 ->
 // I420/YV12) and packed RGB -> the same packed RGB (one plane of 4-byte pixels, opt-in): the reference's
-// plane-scaling fast path (product code, sm_90a).
+// plane-scaling fast path (product code, sm_90a); and the de-interleave of packed RGB -> RGBP / BGRP.
 //
 //   convert_scale_planes            gst-libs/gst/video/video-converter.c:7757-7769
 //   setup_scale                     :7958-8245  (which kernel each plane gets; built on the host, vcs_plan.cpp)
@@ -325,6 +325,46 @@ inline int launch_planes (const PlanesState & st, const VcsBatch & batch, int n,
   }
   const dim3 grid ((wmax + PL_TW - 1) / PL_TW, (hmax + PL_TH - 1) / PL_TH, P.n_planes * n);
   vcs_planes_kernel <<<grid, 256, 0, stream>>> (P, batch);
+  B200_CUDA_TRY (cudaGetLastError ());
+  return B200_OK;
+}
+
+// packed RGB -> planar RGB (RGBP / BGRP).  The reference runs these pairs through its chain without a matrix stage: unpack
+// to ARGB, the scalers, then pack_RGBP / pack_BGRP (gst-libs/gst/video/video-format.c:7496-7536), which store the R, G
+// and B bytes of each ARGB pixel in their own planes and drop the alpha.  The scalers are the packed RGB ones above (4-byte
+// pixels, into a per-handle scratch image); vcs_rgb_deinterleave_kernel is the pack.  YUV inputs never come here: their
+// kernels store the three planes themselves (store_planar_px).
+struct DeintDev {
+  int w, h;
+  unsigned long long soff;       // packed 4-byte pixels: the input frame (unchanged size) or the scaled scratch image
+  int sstride;
+  unsigned sel;                  // plane k takes source byte (sel >> 4k) & 3
+  unsigned long long off[3];
+  int stride[3];
+};
+
+struct DeintBatch {
+  const uint8_t *src[B200_VCS_MAX_BATCH];
+  uint8_t *out[B200_VCS_MAX_BATCH];
+};
+
+// one thread per pixel, 64 x 4 pixels per CTA: each warp reads 128 consecutive source bytes and writes 32 consecutive
+// bytes of every plane
+__global__ void __launch_bounds__ (256)
+vcs_rgb_deinterleave_kernel (const DeintDev D, const DeintBatch frames)
+{
+  const int x = blockIdx.x * 64 + (threadIdx.x & 63), y = blockIdx.y * 4 + (threadIdx.x >> 6);
+  if (x >= D.w || y >= D.h) return;
+  const uint8_t *__restrict__ s = frames.src[blockIdx.z] + D.soff + (size_t) y * D.sstride + 4 * (size_t) x;
+  uint8_t *__restrict__ o = frames.out[blockIdx.z];
+#pragma unroll
+  for (int k = 0; k < 3; k++) o[D.off[k] + (size_t) y * D.stride[k] + x] = s[(D.sel >> (4 * k)) & 3];
+}
+
+inline int launch_rgb_deinterleave (const DeintDev & d, const DeintBatch & b, int n, cudaStream_t stream)
+{
+  const dim3 grid ((d.w + 63) / 64, (d.h + 3) / 4, n);
+  vcs_rgb_deinterleave_kernel <<<grid, 256, 0, stream>>> (d, b);
   B200_CUDA_TRY (cudaGetLastError ());
   return B200_OK;
 }

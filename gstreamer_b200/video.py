@@ -33,6 +33,10 @@ class VideoFormat(enum.IntEnum):
     ARGB = 13
     ABGR = 14
     NV12 = 23
+    # planar 8-bit RGB outputs: one byte plane per component (RGBP: R, G, B; BGRP: B, G, R).  A default-layout frame
+    # whose width is a multiple of 4 is a contiguous (3, height, width) uint8 tensor.
+    RGBP = 99
+    BGRP = 100
     # compositor formats only (planar, little endian, 10 / 12 / 16 bits)
     I420_10LE = 43
     I422_10LE = 45

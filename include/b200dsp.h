@@ -80,6 +80,9 @@ typedef enum {
   B200_VIDEO_FORMAT_xBGR = 10, B200_VIDEO_FORMAT_RGBA = 11, B200_VIDEO_FORMAT_BGRA = 12,
   B200_VIDEO_FORMAT_ARGB = 13, B200_VIDEO_FORMAT_ABGR = 14,
   B200_VIDEO_FORMAT_NV12 = 23, B200_VIDEO_FORMAT_NV21 = 24,
+  /* planar 8-bit RGB outputs (one byte plane per component, a network's CHW input): RGBP = planes R, G, B;
+   * BGRP = planes B, G, R */
+  B200_VIDEO_FORMAT_RGBP = 99, B200_VIDEO_FORMAT_BGRP = 100,
   /* compositor formats only (blend.c PLANAR_YUV_BLEND at 10 / 12 / 16 bits, little endian; Y444 and Y42B above are
    * compositor formats too) */
   B200_VIDEO_FORMAT_I420_10LE = 43, B200_VIDEO_FORMAT_I422_10LE = 45, B200_VIDEO_FORMAT_Y444_10LE = 47,
@@ -146,10 +149,11 @@ typedef struct b200_vcs b200_vcs;
 
 /* Build the per-caps plan (tap tables, matrix, chroma pairing, tiling) and upload it.
  * Format pairs (anything else: B200_ERR_UNSUPPORTED):
- *   NV12 / NV21 / I420 / YV12      -> the eight 4-byte RGB orders, or NV12 / NV21 / I420 / YV12
- *   the eight 4-byte RGB orders    -> the eight 4-byte RGB orders, or NV12 / NV21 / I420 / YV12
- *   YUY2 / UYVY / YVYU             -> the eight 4-byte RGB orders, or NV12 / NV21 / I420 / YV12
- *   Y42B / Y444                    -> the eight 4-byte RGB orders, or NV12 / NV21 / I420 / YV12
+ *   NV12 / NV21 / I420 / YV12      -> the eight 4-byte RGB orders, RGBP / BGRP, or NV12 / NV21 / I420 / YV12
+ *   the eight 4-byte RGB orders    -> the eight 4-byte RGB orders, RGBP / BGRP, or NV12 / NV21 / I420 / YV12
+ *   YUY2 / UYVY / YVYU             -> the eight 4-byte RGB orders, RGBP / BGRP, or NV12 / NV21 / I420 / YV12
+ *   Y42B / Y444                    -> the eight 4-byte RGB orders, RGBP / BGRP, or NV12 / NV21 / I420 / YV12
+ * RGBP / BGRP planes may have any stride >= the width and any offset.
  * A YUV -> YUV pair must name the same colour matrix on both sides (what the element's caps fixation produces).
  * device >= 0: CUDA device ordinal (the element's cuda-device-id property,
  * gst-plugins-bad/sys/nvcodec/gstcudabasetransform.c:89-90).
