@@ -27,11 +27,22 @@
 
 using namespace b200;
 
+// A/B and tuning switches of the converter (DESIGN.md §4.3b), read once when a handle is created
+struct VcsKnobs {
+  bool cross_generic = false;     // B200_CROSS_GENERIC: the 4:2:0 -> other 4:2:0 chain runs the generic kernel
+  bool rgb420_generic = false;    // B200_RGB420_GENERIC: packed RGB / 4:2:2 -> 4:2:0 runs the chain
+  bool l2_v1 = false;             // B200_L2_V1: no second form of the 2:1 kernel
+  bool l2_x4 = false;             // B200_L2_X4 (any value): no second form where it is the only form
+  bool l2_tc = false;             // B200_L2_TC=1: the tensor-core 2:1 kernel (variant 7) by default
+  bool planes_slow = false;       // B200_PLANES_SLOW: the byte-wise plane kernel for every plane
+};
+
 struct b200_vcs {
   VcsPlan plan;
   int device = -1;
+  VcsKnobs knobs;
   VcsDev dev;                     // kernel parameter block (device pointers inside)
-  int variant = 0;
+  int variant = 0;                // the kernel the handle asks for (default or b200_vcs_set_kernel_variant)
   // device tables
   uint32_t *d_hoff = nullptr, *d_voff = nullptr;
   int16_t *d_hcoef = nullptr, *d_vcoef = nullptr, *d_hsum = nullptr, *d_vsum = nullptr;
@@ -76,9 +87,136 @@ struct b200_vcs {
 
 namespace {
 
-size_t frame_bytes (const b200_video_info & i)
+VcsKnobs read_knobs ()
 {
-  return b200_video_info_size (&i);
+  VcsKnobs k;
+  k.cross_generic = getenv ("B200_CROSS_GENERIC") != nullptr;
+  k.rgb420_generic = getenv ("B200_RGB420_GENERIC") != nullptr;
+  k.l2_v1 = getenv ("B200_L2_V1") != nullptr;
+  k.l2_x4 = getenv ("B200_L2_X4") != nullptr;
+  const char *tc = getenv ("B200_L2_TC");
+  k.l2_tc = tc && tc[0] == '1';
+  k.planes_slow = getenv ("B200_PLANES_SLOW") != nullptr;
+  return k;
+}
+
+// the largest power of two up to 16 that divides every frame pointer of a batch
+template <typename T> int alignment (T *const *frames, int n)
+{
+  uintptr_t bits = 16;
+  for (int i = 0; i < n; i++) bits |= (uintptr_t) frames[i];
+  return (int) (bits & (~bits + 1));
+}
+
+// the handle's scratch image: `bytes` per frame for n frames
+int ensure_scratch (b200_vcs * h, size_t bytes, int n)
+{
+  if (n <= h->scratch_frames && bytes == h->scratch_frame_bytes) return B200_OK;
+  B200_CUDA_TRY (cudaFree (h->d_scratch));                          // synchronises with launches still reading it
+  h->d_scratch = nullptr; h->scratch_frames = 0;
+  B200_CUDA_TRY (cudaMalloc ((void **) &h->d_scratch, bytes * n));
+  h->scratch_frames = n; h->scratch_frame_bytes = bytes;
+  return B200_OK;
+}
+
+// What one convert launches after the border fill.  Path::one is a single kernel (Kern); Path::chain is Kern into the
+// scratch image, [the generic kernel for the extra row,] vcs_down420_kernel.
+enum class Path { planes, deint, yuy2, rgb420, chain, one };
+enum Kern { K_GENERIC, K_L2, K_L2V2, K_LIGHT, K_NTAP, K_MMA, K_TC };
+const int kern_variant[] = {0, 1, 1, 2, 3, 6, 7};
+const char *const kern_name[] = {"vcs_generic_kernel", "vcs_lanczos2_kernel", "vcs_lanczos2_v2_kernel", "vcs_light_kernel",
+                                 "vcs_ntap_kernel", "vcs_l2mma_kernel", "vcs_l2tc_kernel"};
+
+struct Route {
+  int status = B200_OK;           // B200_ERR_INVALID_ARG: packed RGB input that is not word aligned
+  Path path = Path::one;
+  Kern kern = K_GENERIC;
+  bool planes_aligned = false;    // Path::planes / deint: the planes' word-wide launches may run (8-byte aligned frames)
+  int kernel_variant = 0;         // b200_vcs_plan_info.kernel_variant
+  const char *name = "";          // b200_vcs_kernel_name
+  int named_variant = 0;          // Path::one / chain: the variant whose kernel `name` is (0: the generic one)
+  int n_launches = 0;             // b200_vcs_plan_info.n_launches_per_convert, the border fill included
+};
+
+// The one place that decides which kernels a convert launches: from the plan, the prepared states, the kernel variant
+// asked for and the alignment of the batch's in / out frames (ain, aout: see alignment ()).  Introspection passes 16.
+// A host-only handle prepares nothing; it reports what the plan selects, with the first form of the 2:1 kernel in
+// place of the second.
+Route select_route (const b200_vcs * h, int variant, int ain, int aout)
+{
+  const VcsPlan & p = h->plan;
+  const bool host = h->device < 0;
+  const int border = p.has_dest && p.fill_border ? 1 : 0;
+  Route r;
+  if (p.planes_mode) {
+    r.kernel_variant = 4;
+    if (p.rgbp_out) {                                               // [the packed RGB scaler into the scratch image ->] de-interleave
+      r.path = Path::deint;
+      r.planes_aligned = ain >= 8;
+      r.name = "vcs_rgb_deinterleave_kernel";
+      r.n_launches = border + 1 + (h->deint_scaled ? plane_launches (h->planes, r.planes_aligned) : 0);
+    } else {
+      r.path = Path::planes;
+      r.planes_aligned = ain >= 8 && aout >= 8;
+      r.name = planes_kernel_name (h->planes);
+      r.n_launches = border + plane_launches (h->planes, r.planes_aligned);
+    }
+    return r;
+  }
+#ifndef B200_CUDA_EMU
+  const bool tc_ready = h->tc.ready;
+#else
+  const bool tc_ready = false;                                    // wgmma: no host emulation
+#endif
+  const bool l2v2 = h->l2v2.ready && h->l2.x4;
+  const bool l2_first = !p.planar && !p.rgbp_out;                 // what the first form of the 2:1 kernel reads and writes
+  const bool ntap_ready = h->ntap.ready || host;
+  if (!p.yuv_out) {
+    if (variant == 6 && h->mma.ready && ain >= 8 && aout >= 4) r.kern = K_MMA;             // 64-bit plane loads
+    else if (variant == 7 && tc_ready && ain >= 16 && aout >= 4) r.kern = K_TC;             // 16-byte cp.async of the luma rows
+    else if (variant == 7 && tc_ready && p.lanczos2_ok && l2_first) r.kern = K_L2;
+    else if (variant == 1 && p.lanczos2_ok && (l2v2 || l2_first || host)) r.kern = l2v2 ? K_L2V2 : K_L2;
+    else if (variant == 2 && p.light_ok && ain >= 4) r.kern = K_LIGHT;                      // 32-bit plane loads
+    else if (variant == 3 && p.ntap_ok && ntap_ready && ain >= 4) r.kern = K_NTAP;
+  }
+  if (r.kern == K_GENERIC && p.rgb_in && ain < 4) r.status = B200_ERR_INVALID_ARG;           // packed pixels: 32-bit loads
+  if (r.kern != K_GENERIC || !p.yuv_out) {
+    r.path = Path::one;
+    r.n_launches = 1;
+  } else if (p.yuy2_420) {
+    r.path = Path::yuy2;
+    r.name = "vcs_yuy2_420_kernel";
+    r.n_launches = 1;
+  } else if (h->rgb420_ok && (h->rgb420_pre != 2 || ain >= 4)) {     // vcs_yuy2_ayuv_kernel reads pixel pairs as words
+    r.path = Path::rgb420;
+    r.name = h->rgb420_pre == 2 ? "vcs_yuy2_ayuv_kernel" : "vcs_rgb420_kernel";
+    r.n_launches = 1 + (h->rgb420_pre ? 1 : 0) + (h->rgb420_scaled ? 1 : 0);
+  } else {
+    // the chain up to the scaled pixels: the 2:1 / light / n-tap kernels (matrix stage off) where the plan allows, else
+    // the generic one
+    r.path = Path::chain;
+    if (variant == 1 && p.lanczos2_ok && ((l2v2 && ain >= 8) || host)) r.kern = l2v2 ? K_L2V2 : K_L2;
+    else if (variant == 2 && p.light_ok && ain >= 4) r.kern = K_LIGHT;
+    else if (variant == 3 && p.ntap_ok && ntap_ready && ain >= 4) r.kern = K_NTAP;
+    r.n_launches = p.extra_row ? 3 : 2;
+  }
+  if (r.path == Path::one || r.path == Path::chain) {
+    r.name = kern_name[r.kern];
+    r.named_variant = kern_variant[r.kern];
+    // B200_CROSS_GENERIC swaps the chain's first launch only: the handle still names the kernel of its variant
+    if (r.path == Path::chain && h->knobs.cross_generic) r.kern = K_GENERIC;
+  }
+  r.kernel_variant = p.yuv_out ? 5 : r.named_variant;
+  r.n_launches += border;
+  return r;
+}
+
+// the variant a new handle runs: the first of 7 (B200_L2_TC=1), 1, 2, 3 whose kernel the route names, else 0
+int default_variant (const b200_vcs * h)
+{
+  for (int v : {7, 1, 2, 3})
+    if ((v != 7 || h->knobs.l2_tc) && select_route (h, v, 16, 16).named_variant == v) return v;
+  return 0;
 }
 
 int upload_axis (const AxisPlan & a, uint32_t **off, int16_t **coef, int16_t **sum, AxisDev * d)
@@ -93,8 +231,6 @@ int upload_axis (const AxisPlan & a, uint32_t **off, int16_t **coef, int16_t **s
   return B200_OK;
 }
 
-int launch_convert (b200_vcs * h, int n, const VcsBatch & batch, cudaStream_t stream);
-
 // packed RGB -> 4:2:0 with every scaler in front of the matrix (the frame does not grow) and no destination rectangle:
 // vcs_rgb420.cuh.  Leaves rgb420_ok false (the generic chain runs) for what the fast kernels decline.
 int prepare_rgb420 (b200_vcs * h)
@@ -102,7 +238,7 @@ int prepare_rgb420 (b200_vcs * h)
   const VcsPlan & p = h->plan;
   h->rgb420_ok = false;
   const bool packed422 = p.in_422_444 && p.ystep == 2;            // YUY2 / UYVY / YVYU
-  if (!(p.rgb_in || packed422) || !p.yuv_out || p.yuy2_420 || getenv ("B200_RGB420_GENERIC")) return B200_OK;
+  if (!(p.rgb_in || packed422) || !p.yuv_out || p.yuy2_420 || h->knobs.rgb420_generic) return B200_OK;
   Rgb420Dev & r = h->rgb420;
   memset (&r, 0, sizeof (r));
   if (p.rgb_in) {
@@ -161,9 +297,34 @@ int prepare_rgb420 (b200_vcs * h)
   return B200_OK;
 }
 
-int launch (b200_vcs * h, int n, const VcsBatch & batch, cudaStream_t stream)
+// one launch of kernel k: the single kernel of Path::one, the chain's first launch (into the scratch image)
+int launch_kern (b200_vcs * h, Kern k, const VcsBatch & batch, int n, cudaStream_t stream)
 {
   const VcsPlan & p = h->plan;
+  switch (k) {
+    case K_L2: return launch_lanczos2 (h->dev, h->l2, batch, n, stream);
+    case K_L2V2: return launch_lanczos2_v2 (h->dev, h->l2, h->l2v2, batch, n, stream, p.rgbp_out);
+    case K_LIGHT: return launch_light (h->dev, p, batch, n, stream);
+    case K_NTAP: return launch_ntap (h->dev, p, h->ntap, batch, n, stream);
+    case K_MMA: return launch_l2mma (h->dev, h->mma, batch, n, stream);
+#ifndef B200_CUDA_EMU
+    case K_TC: return launch_l2tc (h->dev, h->tc, batch, n, stream);
+#endif
+    default: break;
+  }
+  dim3 grid ((p.out.width + p.tile_w - 1) / p.tile_w, (p.out.height + p.tile_h - 1) / p.tile_h, n);
+  if (p.rgbp_out) vcs_generic_kernel<true> <<<grid, 256, p.smem_bytes, stream>>> (h->dev, batch);
+  else vcs_generic_kernel<false> <<<grid, 256, p.smem_bytes, stream>>> (h->dev, batch);
+  B200_CUDA_TRY (cudaGetLastError ());
+  return B200_OK;
+}
+
+int launch_convert (b200_vcs * h, int n, const VcsBatch & batch, cudaStream_t stream)
+{
+  const VcsPlan & p = h->plan;
+  const int ain = alignment (batch.in, n), aout = alignment (batch.out, n);
+  const Route r = select_route (h, h->variant, ain, aout);
+  int st;
   if (p.has_dest && p.fill_border) {
     // border and rectangle are disjoint byte sets: the fill simply goes first on the same stream
     BorderBatch b;
@@ -176,188 +337,199 @@ int launch (b200_vcs * h, int n, const VcsBatch & batch, cudaStream_t stream)
     vcs_border_kernel <<<grid, 256, 0, stream>>> (h->border, b);
     B200_CUDA_TRY (cudaGetLastError ());
   }
-  return launch_convert (h, n, batch, stream);
+  if (r.status != B200_OK) return r.status;
+  switch (r.path) {
+    case Path::planes:
+      return launch_planes (h->planes, batch, n, stream, r.planes_aligned);
+    case Path::deint: {
+      // packed RGB -> RGBP / BGRP: [the packed RGB scaler into the scratch image ->] de-interleave
+      DeintBatch fin;
+      for (int i = 0; i < n; i++) { fin.src[i] = batch.in[i]; fin.out[i] = batch.out[i]; }
+      if (h->deint_scaled) {
+        const size_t frame = (size_t) h->deint.sstride * h->deint.h;
+        if ((st = ensure_scratch (h, frame, n)) != B200_OK) return st;
+        VcsBatch mid;
+        for (int i = 0; i < n; i++) { mid.in[i] = batch.in[i]; mid.out[i] = h->d_scratch + frame * i; fin.src[i] = mid.out[i]; }
+        if ((st = launch_planes (h->planes, mid, n, stream, r.planes_aligned)) != B200_OK) return st;
+      }
+      return launch_rgb_deinterleave (h->deint, fin, n, stream);
+    }
+    case Path::yuy2: {
+      Yuy2Dev y = h->yuy2;
+      Yuy2Batch b;
+      for (int i = 0; i < n; i++) { b.src[i] = batch.in[i]; b.out[i] = batch.out[i]; }
+      if (ain < 16 && y.svec > 1) y.svec = 1;
+      if (ain < 4) y.svec = 0;
+      if (aout < 4) y.wvec = 0;
+      return launch_yuy2_420 (y, b, n, stream);
+    }
+    case Path::rgb420: {
+      // [vcs_rgb2ayuv_kernel / vcs_yuy2_ayuv_kernel ->] [the word-wide scaler ->] matrix + down-sample + pack
+      Rgb420Dev rd = h->rgb420;
+      if (aout < 4) rd.wvec = 0;
+      const int pre = h->rgb420_pre;
+      const int pre_stride = pre == 1 ? h->rgb2ayuv.dstride : pre == 2 ? h->yuy2ayuv.dstride : 0;
+      const size_t pre_bytes = (size_t) pre_stride * p.in.height;
+      const size_t scaled_bytes = h->rgb420_scaled ? (size_t) rd.sstride * p.out.height : 0;
+      const size_t frame = pre_bytes + scaled_bytes;
+      if (frame && (st = ensure_scratch (h, frame, n)) != B200_OK) return st;
+      VcsBatch mid;                                                 // the scaler's view: in = the pre kernel's image or the frame
+      Rgb420Batch fin;
+      for (int i = 0; i < n; i++) { mid.in[i] = batch.in[i]; fin.out[i] = batch.out[i]; }
+      if (pre) {
+        Rgb420Batch pre_b;
+        for (int i = 0; i < n; i++) { pre_b.src[i] = batch.in[i]; pre_b.out[i] = h->d_scratch + frame * i + scaled_bytes; mid.in[i] = pre_b.out[i]; }
+        st = pre == 1 ? launch_rgb2ayuv (h->rgb2ayuv, pre_b, n, stream) : launch_yuy2_ayuv (h->yuy2ayuv, pre_b, n, stream);
+        if (st != B200_OK) return st;
+      }
+      if (h->rgb420_scaled) {
+        for (int i = 0; i < n; i++) { mid.out[i] = h->d_scratch + frame * i; fin.src[i] = mid.out[i]; }
+        if ((st = launch_plane_fast (h->rgb420_scaler, mid, n, stream)) != B200_OK) return st;
+      } else {
+        for (int i = 0; i < n; i++) fin.src[i] = mid.in[i];
+        if (alignment (mid.in, n) < 16) rd.svec = 0;
+      }
+      return launch_rgb420 (rd, fin, n, stream, pre == 0);
+    }
+    case Path::chain: {
+      // launch 1 writes the scaled pixels of every frame to its scratch image, launch 2 down-samples and packs
+      const size_t frame = (size_t) h->down.stride_s * (p.out.height + (p.extra_row ? 1 : 0));
+      if ((st = ensure_scratch (h, frame, n)) != B200_OK) return st;
+      VcsBatch mid;
+      Down420Batch fin;
+      for (int i = 0; i < n; i++) {
+        mid.in[i] = batch.in[i]; mid.out[i] = h->d_scratch + frame * i;
+        fin.scratch[i] = mid.out[i]; fin.out[i] = batch.out[i];
+      }
+      if ((st = launch_kern (h, r.kern, mid, n, stream)) != B200_OK) return st;
+      if (p.extra_row) {
+        // scratch row `oh`: the chain over a one-line view of the frame (its last line, chroma row unfiltered vertically)
+        VcsDev x = h->dev;
+        x.off_y += (unsigned long long) (p.in.height - 1) * x.stride_y;
+        x.off_u += (unsigned long long) ((p.in.height - 1) >> 1) * x.stride_u;
+        x.off_v += (unsigned long long) ((p.in.height - 1) >> 1) * x.stride_v;
+        x.ih = 1; x.oh = 1; x.v.in_size = x.v.out_size = 1;
+        x.off_out = (unsigned long long) p.out.height * x.stride_out;
+        dim3 gx ((p.out.width + p.tile_w - 1) / p.tile_w, 1, n);
+        vcs_generic_kernel<false> <<<gx, 256, p.smem_bytes, stream>>> (x, mid);
+        B200_CUDA_TRY (cudaGetLastError ());
+      }
+      const int cw = (p.out.width + 1) / 2, chh = (p.out.height + 1) / 2;
+      dim3 blk (32, 8), g2 ((cw + 31) / 32, (chh + 7) / 8, n);
+      vcs_down420_kernel <<<g2, blk, 0, stream>>> (h->down, fin);
+      B200_CUDA_TRY (cudaGetLastError ());
+      return B200_OK;
+    }
+    case Path::one:
+      break;
+  }
+  return launch_kern (h, r.kern, batch, n, stream);
 }
 
-int launch_convert (b200_vcs * h, int n, const VcsBatch & batch, cudaStream_t stream)
+// what a device handle uploads and derives for its launches (the handle's device is current)
+int prepare_device (b200_vcs * h)
 {
   const VcsPlan & p = h->plan;
+  int st;
   if (p.planes_mode && p.rgbp_out) {
-    // packed RGB -> RGBP / BGRP: [the packed RGB scaler into the scratch image ->] de-interleave
-    DeintDev d = h->deint;
-    DeintBatch fin;
-    for (int i = 0; i < n; i++) { fin.src[i] = batch.in[i]; fin.out[i] = batch.out[i]; }
-    if (h->deint_scaled) {
-      const size_t frame = (size_t) d.sstride * d.h;
-      if (n > h->scratch_frames || frame != h->scratch_frame_bytes) {
-        B200_CUDA_TRY (cudaFree (h->d_scratch));                    // synchronises with launches still reading it
-        h->d_scratch = nullptr; h->scratch_frames = 0;
-        B200_CUDA_TRY (cudaMalloc ((void **) &h->d_scratch, frame * n));
-        h->scratch_frames = n; h->scratch_frame_bytes = frame;
-      }
-      VcsBatch mid;
-      bool aligned = true;
-      for (int i = 0; i < n; i++) {
-        mid.in[i] = batch.in[i]; mid.out[i] = h->d_scratch + frame * i; fin.src[i] = mid.out[i];
-        aligned = aligned && (((uintptr_t) batch.in[i]) & 7) == 0;
-      }
-      const int s = launch_planes (h->planes, mid, n, stream, aligned);
-      if (s != B200_OK) return s;
+    // packed RGB -> planar RGB: the scaler writes a scratch image of 4-byte pixels (16-byte aligned rows), the
+    // de-interleave reads it - or the input frame itself at an unchanged size
+    DeintDev & d = h->deint;
+    memset (&d, 0, sizeof (d));
+    d.w = p.out.width; d.h = p.out.height; d.sel = p.deint_sel;
+    for (int k = 0; k < 3; k++) { d.off[k] = p.out.offset[k]; d.stride[k] = p.out.stride[k]; }
+    if (!h->deint_scaled) {
+      d.soff = p.in.offset[0]; d.sstride = p.in.stride[0];
+      return B200_OK;
     }
-    return launch_rgb_deinterleave (d, fin, n, stream);
+    VcsPlan sp = p;
+    sp.out.offset[0] = 0; sp.out.stride[0] = (p.out.width * 4 + 15) & ~15;
+    d.soff = 0; d.sstride = sp.out.stride[0];
+    return prepare_planes (sp, &h->planes, h->knobs.planes_slow);
   }
-  if (p.planes_mode) {
-    bool aligned = true;                                            // the word-wide halve / copy path needs 8-byte aligned frames
-    for (int i = 0; i < n; i++) aligned = aligned && ((((uintptr_t) batch.in[i]) | ((uintptr_t) batch.out[i])) & 7) == 0;
-    return launch_planes (h->planes, batch, n, stream, aligned);
+  if (p.planes_mode) return prepare_planes (p, &h->planes, h->knobs.planes_slow);   // YUV -> same YUV family: plane scaling
+  VcsDev & d = h->dev;
+  memset (&d, 0, sizeof (d));
+  d.iw = p.in.width; d.ih = p.in.height; d.ow = p.out.width; d.oh = p.out.height;
+  d.stride_y = p.in.stride[0]; d.stride_c = p.in.stride[1]; d.stride_out = p.out.stride[0];
+  d.off_y = p.in.offset[0]; d.off_c = p.in.offset[1]; d.off_out = p.out.offset[0];
+  d.u_index = p.u_index; d.h_cosited = p.h_cosited; d.v_pairs = p.v_pairs;
+  d.planar = p.planar ? 1 : 0; d.chroma_nearest = p.chroma_nearest ? 1 : 0;
+  if (p.planar) {
+    d.off_u = p.in.offset[p.plane_u]; d.off_v = p.in.offset[p.plane_v];
+    d.stride_u = p.in.stride[p.plane_u]; d.stride_v = p.in.stride[p.plane_v];
+  } else {                                                        // interleaved pairs: both components walk the same rows
+    d.off_u = p.in.offset[1] + p.u_index; d.off_v = p.in.offset[1] + (p.u_index ^ 1);
+    d.stride_u = d.stride_v = p.in.stride[1];
   }
-  if (h->variant == 6 && h->mma.ready) {
-    bool aligned = true;                                            // 64-bit plane loads
-    for (int i = 0; i < n; i++) aligned = aligned && (((uintptr_t) batch.in[i]) & 7) == 0 && (((uintptr_t) batch.out[i]) & 3) == 0;
-    if (aligned) return launch_l2mma (h->dev, h->mma, batch, n, stream);
+  d.cstep = p.planar ? 1 : 2;
+  d.ystep = 1; d.chshift = 1; d.cvshift = 1;
+  if (p.in_422_444) {                                             // capture formats: explicit sample geometry
+    d.off_y = p.in_off_y; d.off_u = p.in_off_u; d.off_v = p.in_off_v;
+    d.stride_u = p.in_stride_u; d.stride_v = p.in_stride_v; d.cstep = p.cstep_in;
+    d.ystep = p.ystep; d.chshift = p.chshift; d.cvshift = p.cvshift;
   }
+  d.h_first = p.h_first; d.matrix_first = p.matrix_first;
+  d.yuv_out = p.yuv_out ? 1 : 0;
+  d.rgb_in = p.rgb_in ? 1 : 0; d.in_sel = p.in_sel;
+  for (int i = 0; i < 3; i++) for (int j = 0; j < 4; j++) d.m[i][j] = p.m_rgb2yuv[i][j];
+  if (p.yuv_out) {                                                // the chain's output is the scratch image
+    d.stride_out = p.out.width * 4; d.off_out = 0;
+    Down420Dev & q = h->down;
+    memset (&q, 0, sizeof (q));
+    q.ow = p.out.width; q.oh = p.out.height; q.stride_s = d.stride_out;
+    q.hmode = p.down_h; q.vavg = p.down_v ? 1 : 0; q.extra_row = p.extra_row ? 1 : 0;
+    q.stride_y = p.out.stride[0]; q.off_y = p.out.offset[0];
+    q.stride_u = p.out.stride[p.out_plane_u]; q.stride_v = p.out.stride[p.out_plane_v];
+    q.cstep = p.out_cstep;
+    q.off_u = p.out.offset[p.out_plane_u] + (p.out_cstep == 2 ? p.out_u_index : 0);
+    q.off_v = p.out.offset[p.out_plane_v] + (p.out_cstep == 2 ? (p.out_u_index ^ 1) : 0);
+    if ((st = prepare_rgb420 (h)) != B200_OK) return st;
+    if (p.yuy2_420) {
+      Yuy2Dev & y = h->yuy2;
+      memset (&y, 0, sizeof (y));
+      const bool uyvy = p.in.format == B200_VIDEO_FORMAT_UYVY;
+      y.w = p.in.width; y.h = p.in.height; y.sstride = p.in.stride[0]; y.soff = p.in.offset[0];
+      y.sel_y = uyvy ? 0x7531 : 0x6420; y.sel_c = uyvy ? 0x6420 : 0x7531;
+      y.svec = ((y.sstride | y.soff) & 15) == 0 ? 2 : (((y.sstride | y.soff) & 3) == 0 ? 1 : 0);
+      y.stride_y = q.stride_y; y.stride_u = q.stride_u; y.stride_v = q.stride_v;
+      y.off_y = q.off_y; y.off_u = q.off_u; y.off_v = q.off_v;
+      y.wvec = ((q.stride_y | q.stride_u | q.stride_v) & 3) == 0 && ((q.off_y | q.off_u | q.off_v) & 3) == 0;
+    }
+  }
+  d.p1 = p.p[0]; d.p2 = p.p[1]; d.p3 = p.p[2]; d.p4 = p.p[3]; d.p5 = p.p[4];
+  d.sel = p.byte_sel[0] | (p.byte_sel[1] << 4) | (p.byte_sel[2] << 8) | (p.byte_sel[3] << 12);
+  d.tile_w = p.tile_w; d.tile_h = p.tile_h; d.max_rows = p.max_rows; d.cols_pitch = p.cols_pitch;
+  d.max_crows = p.max_crows;
+  for (int k = 0; k < 3; k++) {                                   // planar RGB output planes (store_planar_px)
+    d.off_pl[k] = p.rgbp_out ? p.out.offset[k] : 0; d.stride_pl[k] = p.rgbp_out ? p.out.stride[k] : 0;
+  }
+  if ((st = upload_axis (p.h, &h->d_hoff, &h->d_hcoef, &h->d_hsum, &d.h)) != B200_OK ||
+      (st = upload_axis (p.v, &h->d_voff, &h->d_vcoef, &h->d_vsum, &d.v)) != B200_OK ||
+      (st = upload (&h->d_cmode, p.chroma_mode.data (), p.chroma_mode.size ())) != B200_OK)
+    return st;
+  d.chroma_mode = h->d_cmode;
+  if ((st = allow_max_dyn_smem (p.rgbp_out ? vcs_generic_kernel<true> : vcs_generic_kernel<false>)) != B200_OK) return st;
+  if (h->mma_tables.ok && (st = prepare_l2mma (h->mma_tables, &h->mma)) != B200_OK) return st;
+  if (p.lanczos2_ok) {
+    if ((st = prepare_lanczos2 (h->l2_tables, h->dev, &h->l2)) != B200_OK) return st;
+    if (h->l2v2_tables.ok && !h->knobs.l2_v1 && (st = prepare_lanczos2_v2 (h->l2v2_tables, &h->l2v2)) != B200_OK) return st;
 #ifndef B200_CUDA_EMU
-  if (h->variant == 7 && h->tc.ready) {
-    bool aligned = true;                                            // 16-byte cp.async of the luma rows
-    for (int i = 0; i < n; i++) aligned = aligned && (((uintptr_t) batch.in[i]) & 15) == 0 && (((uintptr_t) batch.out[i]) & 3) == 0;
-    if (aligned) return launch_l2tc (h->dev, h->tc, batch, n, stream);
-    if (p.lanczos2_ok && !p.planar && !p.rgbp_out) return launch_lanczos2 (h->dev, h->l2, batch, n, stream);
-  }
+    if ((st = prepare_l2tc (h->tc_tables, &h->tc)) != B200_OK) return st;
 #endif
-  if (h->variant == 1 && p.lanczos2_ok && !p.yuv_out) {
-    if (h->l2v2.ready && h->l2.x4) return launch_lanczos2_v2 (h->dev, h->l2, h->l2v2, batch, n, stream, p.rgbp_out);
-    if (!p.planar && !p.rgbp_out) return launch_lanczos2 (h->dev, h->l2, batch, n, stream);
+  } else if (p.light_ok) {
+    if ((st = allow_max_dyn_smem (light_kernel_for (p))) != B200_OK) return st;
+  } else if (p.ntap_ok) {
+    if ((st = prepare_ntap (p, &h->ntap)) != B200_OK) return st;
   }
-  if (h->variant == 2 && p.light_ok && !p.yuv_out) {
-    // 32-bit plane loads: the frame itself must be word aligned (device allocations always are)
-    bool aligned = true;
-    for (int i = 0; i < n; i++) aligned = aligned && (((uintptr_t) batch.in[i]) & 3) == 0;
-    if (aligned) return launch_light (h->dev, p, batch, n, stream);
-  }
-  if (h->variant == 3 && p.ntap_ok && !p.yuv_out) {
-    bool aligned = true;
-    for (int i = 0; i < n; i++) aligned = aligned && (((uintptr_t) batch.in[i]) & 3) == 0;
-    if (aligned) return launch_ntap (h->dev, p, h->ntap, batch, n, stream);
-  }
-  dim3 grid ((p.out.width + p.tile_w - 1) / p.tile_w, (p.out.height + p.tile_h - 1) / p.tile_h, n);
-  if (p.rgb_in)                                                    // packed pixels are read with 32-bit loads
-    for (int i = 0; i < n; i++) if (((uintptr_t) batch.in[i]) & 3) return B200_ERR_INVALID_ARG;
-  if (p.yuy2_420) {
-    Yuy2Dev y = h->yuy2;
-    Yuy2Batch b;
-    for (int i = 0; i < n; i++) {
-      b.src[i] = batch.in[i]; b.out[i] = batch.out[i];
-      const uintptr_t a = (uintptr_t) batch.in[i];
-      if ((a & 15) && y.svec > 1) y.svec = 1;
-      if (a & 3) y.svec = 0;
-      if (((uintptr_t) batch.out[i]) & 3) y.wvec = 0;
-    }
-    return launch_yuy2_420 (y, b, n, stream);
-  }
-  bool pairs_aligned = true;                                        // vcs_yuy2_ayuv_kernel reads pixel pairs as words
-  if (h->rgb420_pre == 2)
-    for (int i = 0; i < n; i++) pairs_aligned = pairs_aligned && (((uintptr_t) batch.in[i]) & 3) == 0;
-  if (p.yuv_out && h->rgb420_ok && pairs_aligned) {
-    Rgb420Dev r = h->rgb420;
-    Rgb420Batch fin;
-    for (int i = 0; i < n; i++) {
-      fin.out[i] = batch.out[i];
-      if (((uintptr_t) batch.out[i]) & 3) r.wvec = 0;
-    }
-    const int pre = h->rgb420_pre;
-    const int pre_stride = pre == 1 ? h->rgb2ayuv.dstride : pre == 2 ? h->yuy2ayuv.dstride : 0;
-    const size_t pre_bytes = (size_t) pre_stride * p.in.height;
-    const size_t scaled_bytes = h->rgb420_scaled ? (size_t) r.sstride * p.out.height : 0;
-    const size_t frame = pre_bytes + scaled_bytes;
-    if (frame && (n > h->scratch_frames || frame != h->scratch_frame_bytes)) {
-      B200_CUDA_TRY (cudaFree (h->d_scratch));                      // synchronises with launches still reading it
-      h->d_scratch = nullptr; h->scratch_frames = 0;
-      B200_CUDA_TRY (cudaMalloc ((void **) &h->d_scratch, frame * n));
-      h->scratch_frames = n; h->scratch_frame_bytes = frame;
-    }
-    VcsBatch mid;                                                   // the scaler's view: in = the pre kernel's image or the frame
-    for (int i = 0; i < n; i++) mid.in[i] = batch.in[i];
-    if (pre) {
-      Rgb420Batch pre_b;
-      for (int i = 0; i < n; i++) { pre_b.src[i] = batch.in[i]; pre_b.out[i] = h->d_scratch + frame * i + scaled_bytes; mid.in[i] = pre_b.out[i]; }
-      const int s0 = pre == 1 ? launch_rgb2ayuv (h->rgb2ayuv, pre_b, n, stream) : launch_yuy2_ayuv (h->yuy2ayuv, pre_b, n, stream);
-      if (s0 != B200_OK) return s0;
-    }
-    if (h->rgb420_scaled) {
-      for (int i = 0; i < n; i++) { mid.out[i] = h->d_scratch + frame * i; fin.src[i] = mid.out[i]; }
-      const int s1 = launch_plane_fast (h->rgb420_scaler, mid, n, stream);
-      if (s1 != B200_OK) return s1;
-    } else {
-      for (int i = 0; i < n; i++) {
-        fin.src[i] = mid.in[i];
-        if (((uintptr_t) mid.in[i]) & 15) r.svec = 0;
-      }
-    }
-    return launch_rgb420 (r, fin, n, stream, pre == 0);
-  }
-  if (p.yuv_out) {
-    // launch 1 writes the scaled pixels of every frame to its scratch image, launch 2 down-samples and packs
-    const size_t frame = (size_t) h->down.stride_s * (p.out.height + (p.extra_row ? 1 : 0));
-    if (n > h->scratch_frames || frame != h->scratch_frame_bytes) {
-      B200_CUDA_TRY (cudaFree (h->d_scratch));                      // synchronises with launches still reading it
-      h->d_scratch = nullptr; h->scratch_frames = 0;
-      B200_CUDA_TRY (cudaMalloc ((void **) &h->d_scratch, frame * n));
-      h->scratch_frames = n; h->scratch_frame_bytes = frame;
-    }
-    VcsBatch mid;
-    Down420Batch fin;
-    for (int i = 0; i < n; i++) {
-      mid.in[i] = batch.in[i]; mid.out[i] = h->d_scratch + frame * i;
-      fin.scratch[i] = mid.out[i]; fin.out[i] = batch.out[i];
-    }
-    // the chain up to the scaled pixels: the light / n-tap kernels (matrix stage off) where the plan allows, else the generic one
-    bool word_aligned = true;
-    for (int i = 0; i < n; i++) word_aligned = word_aligned && (((uintptr_t) batch.in[i]) & 3) == 0;
-    static const bool slow_chain = getenv ("B200_CROSS_GENERIC") != nullptr;     // A/B knob
-    bool dword_aligned = true;
-    for (int i = 0; i < n; i++) dword_aligned = dword_aligned && (((uintptr_t) batch.in[i]) & 7) == 0;
-    if (!slow_chain && dword_aligned && h->variant == 1 && p.lanczos2_ok && h->l2v2.ready && h->l2.x4) {
-      const int s = launch_lanczos2_v2 (h->dev, h->l2, h->l2v2, mid, n, stream);      // exact 2:1, 8 taps: the headline kernel without its matrix
-      if (s != B200_OK) return s;
-    } else if (!slow_chain && word_aligned && h->variant == 2 && p.light_ok) {
-      const int s = launch_light (h->dev, p, mid, n, stream);
-      if (s != B200_OK) return s;
-    } else if (!slow_chain && word_aligned && h->variant == 3 && p.ntap_ok && h->ntap.ready) {
-      const int s = launch_ntap (h->dev, p, h->ntap, mid, n, stream);
-      if (s != B200_OK) return s;
-    } else {
-      vcs_generic_kernel<false> <<<grid, 256, p.smem_bytes, stream>>> (h->dev, mid);
-      B200_CUDA_TRY (cudaGetLastError ());
-    }
-    if (p.extra_row) {
-      // scratch row `oh`: the chain over a one-line view of the frame (its last line, chroma row unfiltered vertically)
-      VcsDev x = h->dev;
-      x.off_y += (unsigned long long) (p.in.height - 1) * x.stride_y;
-      x.off_u += (unsigned long long) ((p.in.height - 1) >> 1) * x.stride_u;
-      x.off_v += (unsigned long long) ((p.in.height - 1) >> 1) * x.stride_v;
-      x.ih = 1; x.oh = 1; x.v.in_size = x.v.out_size = 1;
-      x.off_out = (unsigned long long) p.out.height * x.stride_out;
-      dim3 gx (grid.x, 1, n);
-      vcs_generic_kernel<false> <<<gx, 256, p.smem_bytes, stream>>> (x, mid);
-      B200_CUDA_TRY (cudaGetLastError ());
-    }
-    const int cw = (p.out.width + 1) / 2, chh = (p.out.height + 1) / 2;
-    dim3 blk (32, 8), g2 ((cw + 31) / 32, (chh + 7) / 8, n);
-    vcs_down420_kernel <<<g2, blk, 0, stream>>> (h->down, fin);
-    B200_CUDA_TRY (cudaGetLastError ());
-    return B200_OK;
-  }
-  if (p.rgbp_out) vcs_generic_kernel<true> <<<grid, 256, p.smem_bytes, stream>>> (h->dev, batch);
-  else vcs_generic_kernel<false> <<<grid, 256, p.smem_bytes, stream>>> (h->dev, batch);
-  B200_CUDA_TRY (cudaGetLastError ());
   return B200_OK;
 }
 
 int ensure_pipeline (b200_vcs * h, int chunk)
 {
   if (h->pipeline_ready && chunk <= h->slot_frames) return B200_OK;
-  h->in_bytes = frame_bytes (h->plan.in);
-  h->out_bytes = frame_bytes (h->plan.frame_out);
+  h->in_bytes = b200_video_info_size (&h->plan.in);
+  h->out_bytes = b200_video_info_size (&h->plan.frame_out);
   if (!h->pipeline_ready) {
     B200_CUDA_TRY (cudaStreamCreateWithFlags (&h->s_h2d, cudaStreamNonBlocking));
     B200_CUDA_TRY (cudaStreamCreateWithFlags (&h->s_run, cudaStreamNonBlocking));
@@ -549,159 +721,39 @@ int b200_vcs_create (const b200_video_info * in, const b200_video_info * out,
       }
     }
   }
-  if (h->plan.planes_mode) {                                       // YUV -> same YUV family: plane scaling
-    h->device = device;
-    h->variant = 4;
-    h->in_bytes = frame_bytes (h->plan.in); h->out_bytes = frame_bytes (h->plan.frame_out);
-    if (device >= 0) {
-      int ndev = b200_device_count ();
-      if (ndev <= 0) { delete h; return ndev < 0 ? ndev : B200_ERR_NO_DEVICE; }
-      if (device >= ndev) { delete h; return B200_ERR_INVALID_ARG; }
-      DeviceGuard g (device);
-      if (!g.ok) { delete h; return B200_ERR_CUDA; }
-      if (h->plan.rgbp_out) {
-        // packed RGB -> planar RGB: the scaler writes a scratch image of 4-byte pixels (16-byte aligned rows), the
-        // de-interleave reads it - or the input frame itself at an unchanged size
-        const VcsPlan & q = h->plan;
-        DeintDev & d = h->deint;
-        memset (&d, 0, sizeof (d));
-        d.w = q.out.width; d.h = q.out.height; d.sel = q.deint_sel;
-        for (int k = 0; k < 3; k++) { d.off[k] = q.out.offset[k]; d.stride[k] = q.out.stride[k]; }
-        h->deint_scaled = q.planes[0].mode == PM_SCALE;
-        if (h->deint_scaled) {
-          VcsPlan sp = q;
-          sp.out.offset[0] = 0; sp.out.stride[0] = (q.out.width * 4 + 15) & ~15;
-          d.soff = 0; d.sstride = sp.out.stride[0];
-          if ((st = prepare_planes (sp, &h->planes)) != B200_OK) { b200_vcs_destroy (h); return st; }
-        } else {
-          d.soff = q.in.offset[0]; d.sstride = q.in.stride[0];
-        }
-      } else if ((st = prepare_planes (h->plan, &h->planes)) != B200_OK) { b200_vcs_destroy (h); return st; }
-    }
-    *handle = h;
-    return B200_OK;
-  }
-  if (h->plan.yuv_out && !h->plan.rgb_in && !h->plan.in_422_444 && !h->plan.has_dest) {
-    // the chain's first launch may be the second form of the exact-2:1 kernel with its matrix stage off
-    h->l2_tables = build_lanczos2_tables (h->plan);
-    h->l2v2_tables = build_lanczos2_v2_tables (h->plan, h->l2_tables);
-    h->plan.lanczos2_ok = h->l2_tables.ok && h->l2v2_tables.ok && !getenv ("B200_L2_V1") && !getenv ("B200_L2_X4") && !getenv ("B200_CROSS_GENERIC");
-  }
-  if (!h->plan.yuv_out && !h->plan.in_422_444) {
-    h->l2_tables = build_lanczos2_tables (h->plan);
-    h->l2v2_tables = build_lanczos2_v2_tables (h->plan, h->l2_tables);
-    // planar (I420 / YV12) input exists in the second form of the kernel only
-    // planar RGB output: the second form only as well; the first form and the tensor forms (variants 6 / 7) decline it
-    const bool v2_only = h->plan.planar || h->plan.rgbp_out;
-    h->plan.lanczos2_ok = h->l2_tables.ok && (!v2_only || (h->l2v2_tables.ok && !getenv ("B200_L2_V1") && !getenv ("B200_L2_X4")));
-    if (!h->plan.rgbp_out) {
-      h->mma_tables = build_l2mma_tables (h->plan);
+  h->knobs = read_knobs ();
+  VcsPlan & p = h->plan;
+  if (!p.planes_mode && !p.in_422_444 && (!p.yuv_out || (!p.rgb_in && !p.has_dest))) {
+    // the exact-2:1 kernel: the one kernel of a packed or planar RGB output, or the first launch of the 4:2:0 chain
+    h->l2_tables = build_lanczos2_tables (p);
+    h->l2v2_tables = build_lanczos2_v2_tables (p, h->l2_tables);
+    // planar (I420 / YV12) input, planar RGB output and the chain (matrix stage off) exist in the second form only;
+    // the first form and the tensor forms (variants 6 / 7) decline planar RGB output
+    const bool v2 = h->l2v2_tables.ok && !h->knobs.l2_v1 && !h->knobs.l2_x4;
+    const bool v2_only = p.planar || p.rgbp_out;
+    p.lanczos2_ok = h->l2_tables.ok && (p.yuv_out ? v2 && !h->knobs.cross_generic : (!v2_only || v2));
+    if (!p.yuv_out && !p.rgbp_out) {
+      h->mma_tables = build_l2mma_tables (p);
 #ifndef B200_CUDA_EMU
-      h->tc_tables = build_l2tc_tables (h->plan, h->l2_tables);
+      h->tc_tables = build_l2tc_tables (p, h->l2_tables);
 #endif
     }
   }
-  const VcsPlan & p = h->plan;
-  if (!p.yuv_out && !p.rgbp_out && ((p.out.stride[0] & 3) || (p.out.offset[0] & 3))) { delete h; return B200_ERR_UNSUPPORTED; }
+  if (!p.planes_mode && !p.yuv_out && !p.rgbp_out && ((p.out.stride[0] & 3) || (p.out.offset[0] & 3))) { delete h; return B200_ERR_UNSUPPORTED; }
   h->device = device;
-  // the kernel this plan will run (also reported for host-only handles: caps negotiation dry-runs, CPU tests)
-  h->variant = h->plan.lanczos2_ok ? 1 : (h->plan.light_ok ? 2 : (h->plan.ntap_ok ? 3 : 0));
+  h->deint_scaled = p.planes_mode && p.rgbp_out && p.planes[0].mode == PM_SCALE;
   if (device >= 0) {
     int ndev = b200_device_count ();
     if (ndev <= 0) { delete h; return ndev < 0 ? ndev : B200_ERR_NO_DEVICE; }
     if (device >= ndev) { delete h; return B200_ERR_INVALID_ARG; }
     DeviceGuard g (device);
     if (!g.ok) { delete h; return B200_ERR_CUDA; }
-    VcsDev & d = h->dev;
-    memset (&d, 0, sizeof (d));
-    d.iw = p.in.width; d.ih = p.in.height; d.ow = p.out.width; d.oh = p.out.height;
-    d.stride_y = p.in.stride[0]; d.stride_c = p.in.stride[1]; d.stride_out = p.out.stride[0];
-    d.off_y = p.in.offset[0]; d.off_c = p.in.offset[1]; d.off_out = p.out.offset[0];
-    d.u_index = p.u_index; d.h_cosited = p.h_cosited; d.v_pairs = p.v_pairs;
-    d.planar = p.planar ? 1 : 0; d.chroma_nearest = p.chroma_nearest ? 1 : 0;
-    if (p.planar) {
-      d.off_u = p.in.offset[p.plane_u]; d.off_v = p.in.offset[p.plane_v];
-      d.stride_u = p.in.stride[p.plane_u]; d.stride_v = p.in.stride[p.plane_v];
-    } else {                                                      // interleaved pairs: both components walk the same rows
-      d.off_u = p.in.offset[1] + p.u_index; d.off_v = p.in.offset[1] + (p.u_index ^ 1);
-      d.stride_u = d.stride_v = p.in.stride[1];
-    }
-    d.cstep = p.planar ? 1 : 2;
-    d.ystep = 1; d.chshift = 1; d.cvshift = 1;
-    if (p.in_422_444) {                                           // capture formats: explicit sample geometry
-      d.off_y = p.in_off_y; d.off_u = p.in_off_u; d.off_v = p.in_off_v;
-      d.stride_u = p.in_stride_u; d.stride_v = p.in_stride_v; d.cstep = p.cstep_in;
-      d.ystep = p.ystep; d.chshift = p.chshift; d.cvshift = p.cvshift;
-    }
-    d.h_first = p.h_first; d.matrix_first = p.matrix_first;
-    d.yuv_out = p.yuv_out ? 1 : 0;
-    d.rgb_in = p.rgb_in ? 1 : 0; d.in_sel = p.in_sel;
-    for (int i = 0; i < 3; i++) for (int j = 0; j < 4; j++) d.m[i][j] = p.m_rgb2yuv[i][j];
-    if (p.yuv_out) {                                              // the chain's output is the scratch image
-      d.stride_out = p.out.width * 4; d.off_out = 0;
-      Down420Dev & q = h->down;
-      memset (&q, 0, sizeof (q));
-      q.ow = p.out.width; q.oh = p.out.height; q.stride_s = d.stride_out;
-      q.hmode = p.down_h; q.vavg = p.down_v ? 1 : 0; q.extra_row = p.extra_row ? 1 : 0;
-      q.stride_y = p.out.stride[0]; q.off_y = p.out.offset[0];
-      q.stride_u = p.out.stride[p.out_plane_u]; q.stride_v = p.out.stride[p.out_plane_v];
-      q.cstep = p.out_cstep;
-      q.off_u = p.out.offset[p.out_plane_u] + (p.out_cstep == 2 ? p.out_u_index : 0);
-      q.off_v = p.out.offset[p.out_plane_v] + (p.out_cstep == 2 ? (p.out_u_index ^ 1) : 0);
-      if ((st = prepare_rgb420 (h)) != B200_OK) { b200_vcs_destroy (h); return st; }
-      if (p.yuy2_420) {
-        Yuy2Dev & y = h->yuy2;
-        memset (&y, 0, sizeof (y));
-        const bool uyvy = p.in.format == B200_VIDEO_FORMAT_UYVY;
-        y.w = p.in.width; y.h = p.in.height; y.sstride = p.in.stride[0]; y.soff = p.in.offset[0];
-        y.sel_y = uyvy ? 0x7531 : 0x6420; y.sel_c = uyvy ? 0x6420 : 0x7531;
-        y.svec = ((y.sstride | y.soff) & 15) == 0 ? 2 : (((y.sstride | y.soff) & 3) == 0 ? 1 : 0);
-        y.stride_y = q.stride_y; y.stride_u = q.stride_u; y.stride_v = q.stride_v;
-        y.off_y = q.off_y; y.off_u = q.off_u; y.off_v = q.off_v;
-        y.wvec = ((q.stride_y | q.stride_u | q.stride_v) & 3) == 0 && ((q.off_y | q.off_u | q.off_v) & 3) == 0;
-      }
-    }
-    d.p1 = p.p[0]; d.p2 = p.p[1]; d.p3 = p.p[2]; d.p4 = p.p[3]; d.p5 = p.p[4];
-    d.sel = p.byte_sel[0] | (p.byte_sel[1] << 4) | (p.byte_sel[2] << 8) | (p.byte_sel[3] << 12);
-    d.tile_w = p.tile_w; d.tile_h = p.tile_h; d.max_rows = p.max_rows; d.cols_pitch = p.cols_pitch;
-    d.max_crows = p.max_crows;
-    for (int k = 0; k < 3; k++) {                                   // planar RGB output planes (store_planar_px)
-      d.off_pl[k] = p.rgbp_out ? p.out.offset[k] : 0; d.stride_pl[k] = p.rgbp_out ? p.out.stride[k] : 0;
-    }
-    if ((st = upload_axis (p.h, &h->d_hoff, &h->d_hcoef, &h->d_hsum, &d.h)) != B200_OK ||
-        (st = upload_axis (p.v, &h->d_voff, &h->d_vcoef, &h->d_vsum, &d.v)) != B200_OK ||
-        (st = upload (&h->d_cmode, p.chroma_mode.data (), p.chroma_mode.size ())) != B200_OK) {
-      b200_vcs_destroy (h);
-      return st;
-    }
-    d.chroma_mode = h->d_cmode;
-    if ((st = allow_max_dyn_smem (p.rgbp_out ? vcs_generic_kernel<true> : vcs_generic_kernel<false>)) != B200_OK) { b200_vcs_destroy (h); return st; }
-    if (h->mma_tables.ok) {
-      st = prepare_l2mma (h->mma_tables, &h->mma);
-      if (st != B200_OK) { b200_vcs_destroy (h); return st; }
-    }
-    if (p.lanczos2_ok) {
-      st = prepare_lanczos2 (h->l2_tables, h->dev, &h->l2);
-      if (st != B200_OK) { b200_vcs_destroy (h); return st; }
-      h->variant = 1;
-      if (h->l2v2_tables.ok && !getenv ("B200_L2_V1")) {            // tuning knob: B200_L2_V1 keeps the first form
-        if ((st = prepare_lanczos2_v2 (h->l2v2_tables, &h->l2v2)) != B200_OK) { b200_vcs_destroy (h); return st; }
-      }
-#ifndef B200_CUDA_EMU
-      if ((st = prepare_l2tc (h->tc_tables, &h->tc)) != B200_OK) { b200_vcs_destroy (h); return st; }
-      { const char *e = getenv ("B200_L2_TC"); if (e && e[0] == '1' && h->tc.ready) h->variant = 7; }   // tuning knob
-#endif
-    } else if (p.light_ok) {
-      if ((st = allow_max_dyn_smem (light_kernel_for (p))) != B200_OK) { b200_vcs_destroy (h); return st; }
-      h->variant = 2;
-    } else if (p.ntap_ok) {
-      st = prepare_ntap (p, &h->ntap);
-      if (st != B200_OK) { b200_vcs_destroy (h); return st; }
-      h->variant = 3;
-    }
+    if ((st = prepare_device (h)) != B200_OK) { b200_vcs_destroy (h); return st; }
   }
-  // variant 6 (mma.sync formulation of the 2:1 kernel) is not timed on the H100 and not the default: kept selectable
-  // through b200_vcs_set_kernel_variant for cross-checks only
+  // the kernel this plan will run (also reported for host-only handles: caps negotiation dry-runs, CPU tests).  Variant 6
+  // (mma.sync formulation of the 2:1 kernel) is not timed on the H100 and not the default: kept selectable through
+  // b200_vcs_set_kernel_variant for cross-checks only
+  h->variant = default_variant (h);
   *handle = h;
   return B200_OK;
 }
@@ -748,7 +800,7 @@ int b200_vcs_convert_batch (b200_vcs * h, int n, const void *const *in_frames,
     b.in[i] = (const uint8_t *) in_frames[i];
     b.out[i] = (uint8_t *) out_frames[i];
   }
-  return launch (h, n, b, (cudaStream_t) cuda_stream);
+  return launch_convert (h, n, b, (cudaStream_t) cuda_stream);
 }
 
 int b200_vcs_convert (b200_vcs * h, const void *in_frame, void *out_frame, void *cuda_stream)
@@ -785,7 +837,7 @@ int b200_vcs_convert_host (b200_vcs * h, int n, const void *const *in_host, void
     }
     B200_CUDA_TRY (cudaEventRecord (h->ev_in[s], h->s_h2d));
     B200_CUDA_TRY (cudaStreamWaitEvent (h->s_run, h->ev_in[s], 0));
-    if ((st = launch (h, m, b, h->s_run)) != B200_OK) return st;
+    if ((st = launch_convert (h, m, b, h->s_run)) != B200_OK) return st;
     B200_CUDA_TRY (cudaEventRecord (h->ev_run[s], h->s_run));
     B200_CUDA_TRY (cudaStreamWaitEvent (h->s_d2h, h->ev_run[s], 0));
     for (int j = 0; j < m; j++)
@@ -828,8 +880,9 @@ int b200_vcs_get_plan_info (const b200_vcs * h, b200_vcs_plan_info * info)
   info->h_first = p.h_first; info->matrix_first = p.matrix_first;
   for (int i = 0; i < 5; i++) info->p[i] = p.p[i];
   info->tile_w = p.tile_w; info->tile_h = p.tile_h; info->smem_bytes = p.smem_bytes;
-  info->kernel_variant = p.yuv_out ? 5 : p.planes_mode ? 4 : h->variant == 7 ? 7 : (h->variant == 6 && h->mma.ready) ? 6 : (h->variant == 1 && p.lanczos2_ok) ? 1 : (h->variant == 2 && p.light_ok) ? 2 : (h->variant == 3 && p.ntap_ok) ? 3 : 0;
-  info->n_launches_per_convert = (p.rgbp_out && p.planes_mode ? (p.planes[0].mode == PM_SCALE ? 2 : 1) : p.yuy2_420 ? 1 : h->rgb420_ok ? (1 + (h->rgb420_pre ? 1 : 0) + (h->rgb420_scaled ? 1 : 0)) : p.yuv_out ? (p.extra_row ? 3 : 2) : 1) + (p.has_dest && p.fill_border ? 1 : 0);
+  const Route r = select_route (h, h->variant, 16, 16);
+  info->kernel_variant = r.kernel_variant;
+  info->n_launches_per_convert = r.n_launches;
   return B200_OK;
 }
 
@@ -868,39 +921,17 @@ int b200_vcs_get_chroma_plan (const b200_vcs * h, uint8_t * mode, size_t len)
 int b200_vcs_set_kernel_variant (b200_vcs * h, int variant)
 {
   if (!h || variant < 0 || (variant > 3 && variant != 6 && variant != 7)) return B200_ERR_INVALID_ARG;
-  if (h->plan.planes_mode || h->plan.yuv_out) return B200_ERR_UNSUPPORTED;   // one kernel only
-  if (variant == 6 && !h->mma.ready) return B200_ERR_UNSUPPORTED;
-#ifndef B200_CUDA_EMU
-  if (variant == 7 && !h->tc.ready) return B200_ERR_UNSUPPORTED;
-#else
-  if (variant == 7) return B200_ERR_UNSUPPORTED;
-#endif
-  if (variant == 3 && !(h->plan.ntap_ok && h->ntap.ready)) return B200_ERR_UNSUPPORTED;
-  if (variant == 1 && !h->plan.lanczos2_ok) return B200_ERR_UNSUPPORTED;
-  if (variant == 2 && !h->plan.light_ok) return B200_ERR_UNSUPPORTED;
+  // eligible: a one-kernel route that takes the variant's kernel on aligned frames.  A host-only handle has no n-tap
+  // tables to run variant 3 with.
+  const Route r = select_route (h, variant, 16, 16);
+  if (r.path != Path::one || r.named_variant != variant || (variant == 3 && h->device < 0)) return B200_ERR_UNSUPPORTED;
   h->variant = variant;
   return B200_OK;
 }
 
 const char *b200_vcs_kernel_name (const b200_vcs * h)
 {
-  if (!h) return "";
-  const VcsPlan & p = h->plan;
-  if (p.planes_mode && p.rgbp_out) return "vcs_rgb_deinterleave_kernel";
-  if (p.planes_mode) {
-    for (int i = 0; i < p.n_planes; i++) if (h->planes.fast[i].ok) return h->planes.fast[i].vfirst ? "vcs_planes_fast_vfirst_kernel" : "vcs_planes_fast_kernel";
-    return "vcs_planes_kernel";
-  }
-  if (p.yuy2_420) return "vcs_yuy2_420_kernel";
-  if (h->rgb420_ok) return h->rgb420_pre == 2 ? "vcs_yuy2_ayuv_kernel" : "vcs_rgb420_kernel";
-  if (h->variant == 6 && h->mma.ready) return "vcs_l2mma_kernel";
-#ifndef B200_CUDA_EMU
-  if (h->variant == 7 && h->tc.ready) return "vcs_l2tc_kernel";
-#endif
-  if ((h->variant == 1 || h->variant == 7) && p.lanczos2_ok) return (h->l2v2.ready && h->l2.x4) ? "vcs_lanczos2_v2_kernel" : "vcs_lanczos2_kernel";
-  if (h->variant == 2 && p.light_ok) return "vcs_light_kernel";
-  if (h->variant == 3 && p.ntap_ok) return "vcs_ntap_kernel";
-  return "vcs_generic_kernel";
+  return h ? select_route (h, h->variant, 16, 16).name : "";
 }
 
 }  // extern "C"

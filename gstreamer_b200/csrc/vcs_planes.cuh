@@ -249,7 +249,8 @@ struct PlanesState {
   bool ready = false;
 };
 
-inline int prepare_planes (const VcsPlan & p, PlanesState * st)
+// slow: the byte-wise kernel for every plane (A/B knob B200_PLANES_SLOW)
+inline int prepare_planes (const VcsPlan & p, PlanesState * st, bool slow)
 {
   memset (&st->params, 0, sizeof (st->params));
   st->params.n_planes = p.n_planes;
@@ -268,7 +269,6 @@ inline int prepare_planes (const VcsPlan & p, PlanesState * st)
     }
     if (q.mode != PM_SCALE) continue;
     {
-      static const bool slow = getenv ("B200_PLANES_SLOW") != nullptr;     // A/B knob: the byte-wise kernel for every plane
       std::vector<int32_t> hp, vp;
       const bool okf = !slow && plan_plane_fast (q, d.sstride, d.src_off, d.dstride, d.dst_off, &st->fast[i], &hp, &vp);
       if (okf) {
@@ -297,22 +297,47 @@ inline void free_planes (PlanesState * st)
   for (int i = 0; i < 3; i++) free_plane_fast (&st->fast[i]);
 }
 
+// plane i runs a launch of its own: a word-wide plan (vcs_planes_fast_kernel) or copy / halve of word-aligned rows
+// (vcs_planes_vec_kernel); both need 8-byte aligned frames (`aligned`)
+inline bool plane_own_launch (const PlanesState & st, int i, bool aligned)
+{
+  const PlaneDev & q = st.params.pl[i];
+  return aligned && (st.fast[i].ok || (q.vec4 && q.mode != PM_SCALE && q.mode != PM_DOUBLE));
+}
+
+// the launches of launch_planes: one per plane with a launch of its own, one vcs_planes_kernel for the rest.  Unprepared
+// (a host-only handle): one vcs_planes_kernel.
+inline int plane_launches (const PlanesState & st, bool aligned)
+{
+  if (!st.ready) return 1;
+  int own = 0;
+  for (int i = 0; i < st.params.n_planes; i++) own += plane_own_launch (st, i, aligned) ? 1 : 0;
+  return own + (own < st.params.n_planes ? 1 : 0);
+}
+
+// the kernel named for a plane-scaling handle: the first plane's word-wide kernel, else the byte-wise one
+inline const char *planes_kernel_name (const PlanesState & st)
+{
+  for (int i = 0; i < st.params.n_planes; i++)
+    if (st.fast[i].ok) return st.fast[i].vfirst ? "vcs_planes_fast_vfirst_kernel" : "vcs_planes_fast_kernel";
+  return "vcs_planes_kernel";
+}
+
 inline int launch_planes (const PlanesState & st, const VcsBatch & batch, int n, cudaStream_t stream, bool aligned)
 {
-  // planes with a word-wide plan run their own launch (32-bit source loads: word-aligned frames, which `aligned` implies)
   PlanesParams P;
   memset (&P, 0, sizeof (P));
   for (int i = 0; i < st.params.n_planes; i++) {
     const PlaneDev & q = st.params.pl[i];
-    if (st.fast[i].ok && aligned) {
+    if (!plane_own_launch (st, i, aligned)) {
+      P.pl[P.n_planes++] = q;
+    } else if (st.fast[i].ok) {
       const int s = launch_plane_fast (st.fast[i], batch, n, stream);
       if (s != B200_OK) return s;
-    } else if (aligned && q.vec4 && q.mode != PM_SCALE && q.mode != PM_DOUBLE) {
+    } else {
       const dim3 grid ((((q.ow * q.ne) >> 2) + 63) / 64, (q.oh + 3) / 4, n);
       vcs_planes_vec_kernel <<<grid, 256, 0, stream>>> (q, batch);
       B200_CUDA_TRY (cudaGetLastError ());
-    } else {
-      P.pl[P.n_planes++] = st.params.pl[i];
     }
   }
   if (P.n_planes == 0) return B200_OK;

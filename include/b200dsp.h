@@ -196,7 +196,7 @@ typedef struct {
                                   * 6 = lanczos 2:1 with mma.sync FIRs (cross-check only: set_kernel_variant; not timed on H100),
                                   * 7 = lanczos 2:1 with both FIR passes as wgmma s8 x u8 banded products on the tensor cores
                                   *     (bit-exact; set_kernel_variant(7) or B200_L2_TC=1 - not the default, see DESIGN.md) */
-  int32_t n_launches_per_convert;
+  int32_t n_launches_per_convert; /* kernel launches of one convert on 16-byte aligned frames, the border fill included */
 } b200_vcs_plan_info;
 int b200_vcs_get_plan_info (const b200_vcs * h, b200_vcs_plan_info * info);
 /* copy out the integer tap tables: dir 0 = horizontal, 1 = vertical.
@@ -208,9 +208,11 @@ int b200_vcs_get_taps (const b200_vcs * h, int dir, uint32_t * offsets, int16_t 
 int b200_vcs_get_matrix (const b200_vcs * h, int32_t im[16]);
 /* per input line chroma pairing mode (0 own row, 1 first of pair, 2 second of pair) */
 int b200_vcs_get_chroma_plan (const b200_vcs * h, uint8_t * mode, size_t len);
-/* force a kernel variant (0 generic, 1-3 the fast kernels, 6 the tensor-path 2:1 kernel, each if eligible); for A/B tests */
+/* force a kernel variant (0 generic, 1-3 the fast kernels, 6 the mma.sync and 7 the wgmma form of the 2:1 kernel, each
+ * if eligible: B200_ERR_UNSUPPORTED otherwise, and for plane scaling and 4:2:0 outputs); for A/B tests */
 int b200_vcs_set_kernel_variant (b200_vcs * h, int variant);
-/* name of the __global__ function b200_vcs_convert launches for this handle (what a profiler's launch list shows) */
+/* name of the __global__ function b200_vcs_convert launches for this handle on 16-byte aligned frames (what a profiler's
+ * launch list shows; the n-tap and plane launchers may pick a vcs_ntap_vfirst / vcs_planes_vec form of the named kernel) */
 const char *b200_vcs_kernel_name (const b200_vcs * h);
 
 /* ------------------------------------------------------------------ compositor */

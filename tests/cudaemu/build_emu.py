@@ -1,15 +1,18 @@
 #!/usr/bin/env python
 """tests/cudaemu/build_emu.py — TEST INFRASTRUCTURE.
 
-Builds tests/cudaemu/_build/libb200emu.so: the product's convert+scale glue (vcs.cu), its host plan builder and the
-kernels that need neither PTX nor warp shuffles (vcs_generic_kernel, vcs_planes_kernel, vcs_down420_kernel,
-vcs_border_kernel) compiled with g++ against the stand-in runtime in emu/.  The sources are the product's own files,
-patched textually only where CUDA syntax has no C++ spelling:
-    kernel <<<grid, block, smem, stream>>> (args);   ->   b200emu::launch (grid, block, smem, [&] { kernel (args); });
+Builds tests/cudaemu/_build/libb200emu.so: the product's convert+scale glue (vcs.cu), its host plan builder and its
+kernels except the wgmma one (vcs_l2tc_kernel) compiled with g++ against the stand-in runtime in emu/ (warp shuffles and
+mma.sync have stand-ins there).  The sources are the product's own files, patched textually only where CUDA syntax has
+no C++ spelling:
+    kernel <<<grid, block, smem, stream>>> (args);   ->   b200emu::launch (grid, block, smem, [&] { kernel (args); },
+                                                                           "kernel", (const void *) kernel);
     extern __shared__ ... smem[];                    ->   uint8_t *smem = b200emu::dyn_smem;
     __shared__ T x[N];                               ->   static T x[N];
-The library exports the same b200_vcs_* C-ABI; "device pointers" are host pointers.  It exists so that kernel indexing
-and integer arithmetic can be checked against the oracle without a GPU — it is never loaded by gstreamer_b200."""
+The library exports the same b200_vcs_* C-ABI; "device pointers" are host pointers.  In record-only mode
+(b200emu_set_record_only) a launch runs no block and appends the kernel's name, with its template arguments, to a log
+that b200emu_launch_log reads.  It exists so that kernel indexing and integer arithmetic, and which kernels each
+configuration launches, can be checked without a GPU — it is never loaded by gstreamer_b200."""
 import hashlib
 import os
 import re
@@ -47,7 +50,8 @@ def patch(text):
         name, cfg, args = m.group(1), m.group(2), m.group(3)
         parts = split_top(cfg)
         assert len(parts) == 4, cfg
-        return f"b200emu::launch ({parts[0]}, {parts[1]}, {parts[2]}, [&] {{ {name} ({args}); }});"
+        return (f"b200emu::launch ({parts[0]}, {parts[1]}, {parts[2]}, [&] {{ {name} ({args}); }}, "
+                f"\"{name}\", (const void *) {name});")
     text, n = LAUNCH.subn(repl, text)
     text = re.sub(r"extern __shared__ __align__ \((?:16|128)\) (\w+) (\w+)\[\];", r"\1 *\2 = (\1 *) b200emu::dyn_smem;", text)
     text = re.sub(r"(^|\n)(\s*)__shared__ ", r"\1\2static ", text)

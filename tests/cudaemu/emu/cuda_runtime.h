@@ -5,8 +5,7 @@
 // and have their indexing and integer arithmetic checked against the oracle on a machine without a GPU.  "Device
 // memory" is host memory; a launch runs the blocks of the grid one after another, each block as real threads with a
 // barrier behind __syncthreads().  Nothing in gstreamer_b200/ loads the library built from this; libb200dsp.so has no
-// CPU fallback.  Kernels that use PTX or warp shuffles (the lanczos2 / light / n-tap fast kernels, the audio and
-// compositor kernels) are not emulated.
+// CPU fallback.  Warp shuffles and mma.sync have stand-ins below; the wgmma kernel (vcs_l2tc.cuh) is not emulated.
 #pragma once
 
 #include <pthread.h>
@@ -47,8 +46,9 @@ extern thread_local dim3 blockDim, gridDim;
 namespace b200emu {
 extern uint8_t *dyn_smem;         // the launch's dynamic shared memory: a heap block of exactly the requested size
 void barrier ();
-// runs body once per thread of every block of the grid
-void launch (dim3 grid, dim3 block, size_t smem_bytes, const std::function<void ()> & body);
+// runs body once per thread of every block of the grid; in record-only mode it appends the kernel's name to the launch
+// log instead.  `name` is the kernel as the launch site spells it; `fn` resolves it to its instantiation.
+void launch (dim3 grid, dim3 block, size_t smem_bytes, const std::function<void ()> & body, const char *name, const void *fn);
 }
 
 inline void __syncthreads () { b200emu::barrier (); }

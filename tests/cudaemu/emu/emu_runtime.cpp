@@ -5,8 +5,12 @@
 // separates consecutive blocks (shared memory is reused).
 #include "cuda_runtime.h"
 
+#include <cxxabi.h>
+#include <dlfcn.h>
+
 #include <condition_variable>
 #include <mutex>
+#include <string>
 
 thread_local uint3_emu threadIdx, blockIdx;
 thread_local dim3 blockDim, gridDim;
@@ -126,8 +130,38 @@ static void *thread_main (void *arg)
   return nullptr;
 }
 
-void launch (dim3 grid, dim3 block, size_t smem_bytes, const std::function<void ()> & body)
+static std::string g_log;                      // kernels launched in record-only mode, one per line
+static bool g_record_only = false;
+
+// the instantiation `fn` points at, without namespace, return type and parameters ("vcs_generic_kernel<false>"); the
+// launch site's spelling where the symbol is not exported (a function pointer's variable name, e.g. "fn")
+static std::string kernel_label (const char *name, const void *fn)
 {
+  Dl_info info;
+  if (!dladdr (fn, &info) || !info.dli_sname || info.dli_saddr != fn) return name;
+  int status = -1;
+  char *d = abi::__cxa_demangle (info.dli_sname, nullptr, nullptr, &status);
+  if (status != 0 || !d) { free (d); return name; }
+  const std::string s (d);
+  free (d);
+  size_t start = 0, end = s.size ();
+  int depth = 0;
+  for (size_t i = 0; i < s.size (); i++) {
+    if (s[i] == '<') depth++;
+    else if (s[i] == '>') depth--;
+    else if (depth == 0 && s[i] == '(') { end = i; break; }
+    else if (depth == 0 && (s[i] == ' ' || s.compare (i, 2, "::") == 0)) start = i + (s[i] == ' ' ? 1 : 2);
+  }
+  return s.substr (start, end - start);
+}
+
+void launch (dim3 grid, dim3 block, size_t smem_bytes, const std::function<void ()> & body, const char *name, const void *fn)
+{
+  if (g_record_only) {
+    g_log += kernel_label (name, fn);
+    g_log += '\n';
+    return;
+  }
   const unsigned nt = block.x * block.y * block.z;
   // exactly the requested bytes (rounded to 16): an address sanitizer build then catches a kernel that runs past them
   uint8_t *smem = (uint8_t *) aligned_alloc (16, std::max<size_t> (16, (smem_bytes + 15) & ~(size_t) 15));
@@ -152,3 +186,13 @@ void launch (dim3 grid, dim3 block, size_t smem_bytes, const std::function<void 
 }
 
 }  // namespace b200emu
+
+extern "C" {
+
+// the kernels launched since the last clear, one name per line (valid until the next launch or clear)
+const char *b200emu_launch_log () { return b200emu::g_log.c_str (); }
+void b200emu_clear_launch_log () { b200emu::g_log.clear (); }
+// on: launches are logged and no block runs (route tests); off (the default): launches run and are not logged
+void b200emu_set_record_only (int on) { b200emu::g_record_only = on != 0; }
+
+}

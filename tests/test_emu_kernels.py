@@ -73,7 +73,7 @@ def run(emu, fi, fo, size, method, frame, colorimetry=None, dest=None, border=0x
     assert st == 0, (st, fi, fo, size)
     try:
         if force_generic:
-            emu.b200_vcs_set_kernel_variant(h, 0)    # the fast kernels (PTX, shuffles) are not emulated
+            emu.b200_vcs_set_kernel_variant(h, 0)    # the generic kernel (the fast kernels have tests of their own)
         out = np.full(emu.b200_video_info_size(C.byref(oi)), 0x5A, dtype=np.uint8)
         src = np.ascontiguousarray(frame)
         assert emu.b200_vcs_convert(h, src.ctypes.data, out.ctypes.data, None) == 0
@@ -201,6 +201,11 @@ def test_planes_fast_kernel(emu, size, monkeypatch):
         frame = frame_for(fi, iw, ih, 5)
         for method in (0, 1, 3, 9, 4):
             check(run(emu, fi, fo, size, method, frame), expected(fi, fo, size, method, frame), f"{fi}->{fo} m{method}")
+    monkeypatch.setenv("B200_PLANES_SLOW", "1")                # read by each new handle
+    for fi, fo in [("NV12", "NV12"), ("I420", "YV12")]:
+        frame = frame_for(fi, iw, ih, 6)
+        for method in (1, 3):
+            check(run(emu, fi, fo, size, method, frame), expected(fi, fo, size, method, frame), f"slow {fi}->{fo} m{method}")
 
 
 # ---- 2b. the fast kernels (device-verified; here as a CPU regression net for future changes to them) -----------------------
