@@ -11,7 +11,8 @@
 //    sample word as the second source), which puts the four output columns' windows on the 0/2/4/6 byte grid: 10 IDP.4A per
 //    line and channel instead of 12 (two tap words are all zero and never issued).  Luma comes from memory on the 8-byte
 //    grid and keeps 12.
-//  * the next item's seven loads are issued before the current item's arithmetic (the H phase spent 2.3 stalled warps per
+//  * a warp's line groups are consecutive: the chroma row two groups share is up-sampled once and carried in registers, and
+//    the next group's six loads are issued before the current group's arithmetic (the H phase spent 2.3 stalled warps per
 //    issue waiting for its loads)
 //  * V phase: accumulators preset to 128 - 32768 and packed with signed 16-bit saturation, so byte 1 of each half IS the
 //    rounded, saturated sample minus 128 - the bias xor and the byte-gather PRMT go, the third channel of two pixels shares
@@ -63,16 +64,17 @@ __device__ __forceinline__ unsigned pack_sat_s16x2 (int a, int b)     // { sat_s
   } while (0)
 
 // SEL: the output format's byte selector (VcsDev::sel) when known at compile time, -1: applied with a PRMT per pixel.
-// PF: 1 the next H item's loads are issued before this item's arithmetic, 2 only its chroma rows, 0 neither.
+// PF: 0, nothing else exists any more (the H phase always loads one line group ahead); MINB, PF, TH and NT stay in the
+// argument list because the instantiation's full name is what the recorded route table (tests/golden/vcs_routes.json) holds.
 // PLANAR: I420 / YV12 input - a chroma row is one 32-bit word from each of the U and V planes (already de-interleaved).
 // YUVOUT: 4:2:0 output through the chain (VcsDev::yuv_out): no matrix stage, {255, Y, U, V} pixels for vcs_down420_kernel.
 // PLOUT: planar RGB output (RGBP / BGRP): the packed pixel's bytes 0..2 go to three planes (store_planar_px).
-// TH x NT: output rows per tile and threads per CTA (60 x 256 at 4 CTAs per SM, or 124 x 512 at 2: 256 of 254 filtered lines used
-// instead of 128 of 126).
+// TH x NT: output rows per tile and threads per CTA: 60 x 256 at MINB = 4 CTAs per SM (124 x 512 at 2 measured slower on H100).
 template <int MINB, int SEL, int PF, int TH = 60, int NT = L2_THREADS, bool PLANAR = false, bool YUVOUT = false, bool PLOUT = false>
 __global__ void __launch_bounds__ (NT, MINB)
 vcs_lanczos2_v2_kernel (const VcsDev P, const Lanczos2Dev L, const Lanczos2V2Dev K, const VcsBatch frames)
 {
+  static_assert (PF == 0, "one H-phase load schedule");
   constexpr int NWC = 1, NWARP = NT / 32;
   constexpr int L2_NG = L2Shape<TH, NWC>::NG, L2_TW = L2Shape<TH, NWC>::TW, L2_TWP = L2Shape<TH, NWC>::TWP;
 
@@ -96,7 +98,6 @@ vcs_lanczos2_v2_kernel (const VcsDev P, const Lanczos2Dev L, const Lanczos2V2Dev
   // bottom border keep the constant taps and clamp their line / chroma-row indices
   const bool edge_tile = x0 == 0 || x0 + L2_TW + 4 >= P.ow;
   const bool edge_rows = R0 < 0 || R0 + 4 * ng > P.ih;
-  struct Raw { uint2 c[3]; uint2 y[4]; };
 
 #define L2_PACK4X(A, c) __byte_perm (pack_sat_u16x2 (A[1][c], A[0][c]), pack_sat_u16x2 (A[3][c], A[2][c]), 0x7531)
 #define L2_PACK4P(A, c) pack_sat2 (sra6 (A[1][c]), sra6 (A[0][c]), pack_sat2 (sra6 (A[3][c]), sra6 (A[2][c]), 0u))
@@ -177,49 +178,44 @@ vcs_lanczos2_v2_kernel (const VcsDev P, const Lanczos2Dev L, const Lanczos2V2Dev
   } else {
     // interior tiles: uniform taps times 4 from the constant bank, chroma on the shifted grid, loads one item ahead
     const int xb = 2 * (x0 + (lane - 1) * 4);                    // byte column of the lane's 8 input pixels
-    auto h_load_c = [&] (auto clamp_tag, int g, uint2 (&c)[3]) {
-      const int m2 = (R0 + 4 * g - 1) >> 1;
-      if (PLANAR) {                                              // c[k].x = 4 U samples, c[k].y = 4 V samples
-#pragma unroll
-        for (int k = 0; k < 3; k++) {
-          const int cr = decltype (clamp_tag)::value ? min (max (m2 + k, 0), crows - 1) : m2 + k;
-          c[k].x = __ldg ((const unsigned *) (plane_u + (ptrdiff_t) cr * P.stride_u + (xb >> 1)));
-          c[k].y = __ldg ((const unsigned *) (plane_v + (ptrdiff_t) cr * P.stride_v + (xb >> 1)));
-        }
-      } else if (decltype (clamp_tag)::value) {
-#pragma unroll
-        for (int k = 0; k < 3; k++)
-          c[k] = __ldg ((const uint2 *) (plane_c + (size_t) min (max (m2 + k, 0), crows - 1) * P.stride_c + xb));
-      } else {
-        const uint8_t *pc = plane_c + (ptrdiff_t) m2 * P.stride_c + xb;
-#pragma unroll
-        for (int k = 0; k < 3; k++) { c[k] = __ldg ((const uint2 *) pc); pc += P.stride_c; }
+    struct Raw { uint2 c[2]; uint2 y[4]; };
+    // one chroma row: 8 interleaved bytes, or (PLANAR) .x = 4 U samples, .y = 4 V samples
+    auto h_load_c = [&] (auto clamp_tag, int row) {
+      const int cr = decltype (clamp_tag)::value ? min (max (row, 0), crows - 1) : row;
+      if (PLANAR) {
+        uint2 c;
+        c.x = __ldg ((const unsigned *) (plane_u + (ptrdiff_t) cr * P.stride_u + (xb >> 1)));
+        c.y = __ldg ((const unsigned *) (plane_v + (ptrdiff_t) cr * P.stride_v + (xb >> 1)));
+        return c;
       }
+      return __ldg ((const uint2 *) (plane_c + (ptrdiff_t) cr * P.stride_c + xb));
     };
-    auto h_load_y = [&] (auto clamp_tag, int g, uint2 (&y)[4]) {
-      const int y0 = R0 + 4 * g;
+    // what line group g needs beyond the chroma row it shares with group g - 1: two chroma rows and four lines
+    auto h_load = [&] (auto clamp_tag, int g, Raw & r) {
+      const int y0 = R0 + 4 * g, m2 = (y0 - 1) >> 1;
+      r.c[0] = h_load_c (clamp_tag, m2 + 1); r.c[1] = h_load_c (clamp_tag, m2 + 2);
       if (decltype (clamp_tag)::value) {
 #pragma unroll
-        for (int r = 0; r < 4; r++)
-          y[r] = __ldg ((const uint2 *) (plane_y + (size_t) min (max (y0 + r, 0), P.ih - 1) * P.stride_y + xb));
+        for (int k = 0; k < 4; k++)
+          r.y[k] = __ldg ((const uint2 *) (plane_y + (size_t) min (max (y0 + k, 0), P.ih - 1) * P.stride_y + xb));
       } else {
         const uint8_t *py = plane_y + (ptrdiff_t) y0 * P.stride_y + xb;
 #pragma unroll
-        for (int r = 0; r < 4; r++) { y[r] = __ldg ((const uint2 *) py); py += P.stride_y; }
+        for (int k = 0; k < 4; k++) { r.y[k] = __ldg ((const uint2 *) py); py += P.stride_y; }
       }
     };
-    auto h_item = [&] (int g, const uint2 (&rc)[3], const uint2 (&ry)[4]) {
-      unsigned ulo[3], uhi[3], vlo[3], vhi[3];                   // [o0 e1 o1 e2], [o2 e3 o3 e4]: pixels 8L+1 .. 8L+8
-#pragma unroll
-      for (int k = 0; k < 3; k++) {
-        const unsigned ue = PLANAR ? rc[k].x : __byte_perm (rc[k].x, rc[k].y, selU), ve = PLANAR ? rc[k].y : __byte_perm (rc[k].x, rc[k].y, selV);
-        unsigned un = __shfl_down_sync (0xffffffffu, ue, 1), vn = __shfl_down_sync (0xffffffffu, ve, 1);
-        un = __byte_perm (ue, un, 0x4321);
-        vn = __byte_perm (ve, vn, 0x4321);
-        const unsigned uo = avg_ceil4 (ue, un), vo = avg_ceil4 (ve, vn);
-        ulo[k] = __byte_perm (uo, un, 0x5140); uhi[k] = __byte_perm (uo, un, 0x7362);
-        vlo[k] = __byte_perm (vo, vn, 0x5140); vhi[k] = __byte_perm (vo, vn, 0x7362);
-      }
+    // a chroma row up-sampled horizontally: [o0 e1 o1 e2], [o2 e3 o3 e4] of each plane, pixels 8L+1 .. 8L+8
+    auto h_up = [&] (const uint2 c, unsigned & ulo, unsigned & uhi, unsigned & vlo, unsigned & vhi) {
+      const unsigned ue = PLANAR ? c.x : __byte_perm (c.x, c.y, selU), ve = PLANAR ? c.y : __byte_perm (c.x, c.y, selV);
+      unsigned un = __shfl_down_sync (0xffffffffu, ue, 1), vn = __shfl_down_sync (0xffffffffu, ve, 1);
+      un = __byte_perm (ue, un, 0x4321);
+      vn = __byte_perm (ve, vn, 0x4321);
+      const unsigned uo = avg_ceil4 (ue, un), vo = avg_ceil4 (ve, vn);
+      ulo = __byte_perm (uo, un, 0x5140); uhi = __byte_perm (uo, un, 0x7362);
+      vlo = __byte_perm (vo, vn, 0x5140); vhi = __byte_perm (vo, vn, 0x7362);
+    };
+    auto h_item = [&] (int g, const unsigned (&ulo)[3], const unsigned (&uhi)[3], const unsigned (&vlo)[3], const unsigned (&vhi)[3],
+        const uint2 (&ry)[4]) {
       unsigned U[4][2], V[4][2];
       L2_VPAIRS (U, ulo, uhi);
       L2_VPAIRS (V, vlo, vhi);
@@ -243,35 +239,28 @@ vcs_lanczos2_v2_kernel (const VcsDev P, const Lanczos2Dev L, const Lanczos2V2Dev
       }
       L2_STOREV (0, acc, L2_PACK4X);
     };
+    // a warp takes a run of consecutive line groups: the last chroma row of a group (rows m2, m2 + 1, m2 + 2) is the first of
+    // the next (m2 + 2 ..), so its up-sampled words stay in registers and every group after the run's first loads and
+    // up-samples two rows instead of three (a clamped row index that repeats is still the same row)
     auto h_run = [&] (auto clamp_tag) {
-      if (PF == 1) {                                             // all seven loads one item ahead
-        Raw ra, rb;
-        if (warp < ng) { h_load_c (clamp_tag, warp, ra.c); h_load_y (clamp_tag, warp, ra.y); }
-        for (int g = warp; g < ng; g += 2 * NWARP) {             // ng < L2_NG in the frame's last, short tile row
-          if (g + NWARP < ng) { h_load_c (clamp_tag, g + NWARP, rb.c); h_load_y (clamp_tag, g + NWARP, rb.y); }
-          h_item (g, ra.c, ra.y);
-          if (g + 2 * NWARP < ng) { h_load_c (clamp_tag, g + 2 * NWARP, ra.c); h_load_y (clamp_tag, g + 2 * NWARP, ra.y); }
-          if (g + NWARP < ng) h_item (g + NWARP, rb.c, rb.y);
-        }
-      } else if (PF == 2) {                                      // the chroma rows (needed first) one item ahead
-        uint2 ca[3], cb[3], y[4];
-        if (warp < ng) h_load_c (clamp_tag, warp, ca);
-        for (int g = warp; g < ng; g += 2 * NWARP) {
-          h_load_y (clamp_tag, g, y);
-          if (g + NWARP < ng) h_load_c (clamp_tag, g + NWARP, cb);
-          h_item (g, ca, y);
-          if (g + NWARP < ng) {
-            h_load_y (clamp_tag, g + NWARP, y);
-            if (g + 2 * NWARP < ng) h_load_c (clamp_tag, g + 2 * NWARP, ca);
-            h_item (g + NWARP, cb, y);
-          }
-        }
-      } else {
-        for (int g = warp; g < ng; g += NWARP) {
-          Raw r;
-          h_load_c (clamp_tag, g, r.c); h_load_y (clamp_tag, g, r.y);
-          h_item (g, r.c, r.y);
-        }
+      const int per = (ng + NWARP - 1) / NWARP;                  // ng < L2_NG in the frame's last, short tile row
+      const int g0 = warp * per, g1 = min (ng, g0 + per);
+      if (g0 >= g1) return;
+      // every load is issued before the arithmetic that precedes its use: the run's first chroma row and first group before
+      // anything else, then each next group's six loads before the current group's FIRs
+      const uint2 c0 = h_load_c (clamp_tag, (R0 + 4 * g0 - 1) >> 1);
+      Raw r;
+      h_load (clamp_tag, g0, r);
+      unsigned ulo[3], uhi[3], vlo[3], vhi[3];
+      h_up (c0, ulo[2], uhi[2], vlo[2], vhi[2]);
+      for (int g = g0; g < g1; g++) {
+        ulo[0] = ulo[2]; uhi[0] = uhi[2]; vlo[0] = vlo[2]; vhi[0] = vhi[2];
+        h_up (r.c[0], ulo[1], uhi[1], vlo[1], vhi[1]);
+        h_up (r.c[1], ulo[2], uhi[2], vlo[2], vhi[2]);
+        Raw n;
+        if (g + 1 < g1) h_load (clamp_tag, g + 1, n);
+        h_item (g, ulo, uhi, vlo, vhi, r.y);
+        r = n;
       }
     };
     if (edge_rows) h_run (std::true_type {}); else h_run (std::false_type {});
@@ -435,11 +424,12 @@ inline int prepare_lanczos2_v2 (const Lanczos2V2Tables & t, Lanczos2V2State * st
   return B200_OK;
 }
 
-template <int SEL, int PF, int MINB = 4, int TH = 60, int NT = L2_THREADS, bool PLANAR = false, bool YUVOUT = false, bool PLOUT = false>
+template <int SEL, bool PLANAR = false, bool YUVOUT = false, bool PLOUT = false>
 inline int launch_lanczos2_v2_sel (const VcsDev & d, const Lanczos2State & st, const Lanczos2V2State & v2, const VcsBatch & batch,
     int n, cudaStream_t stream)
 {
-  auto kern = vcs_lanczos2_v2_kernel<MINB, SEL, PF, TH, NT, PLANAR, YUVOUT, PLOUT>;
+  constexpr int TH = 60, NT = L2_THREADS;
+  auto kern = vcs_lanczos2_v2_kernel<4, SEL, 0, TH, NT, PLANAR, YUVOUT, PLOUT>;
   static bool attr_done[16] = {false};
   int dev = 0; cudaGetDevice (&dev);
   if (!attr_done[dev & 15]) {
@@ -458,26 +448,25 @@ inline int launch_lanczos2_v2 (const VcsDev & d, const Lanczos2State & st, const
   if (planar_out) {                               // RGBP (sel of RGBx) / BGRP (sel of BGRx)
     const bool bgr = d.sel == 0x0123u;
     if (d.planar)
-      return bgr ? launch_lanczos2_v2_sel<0x0123, 0, 4, 60, L2_THREADS, true, false, true> (d, st, v2, batch, n, stream)
-                 : launch_lanczos2_v2_sel<0x0321, 0, 4, 60, L2_THREADS, true, false, true> (d, st, v2, batch, n, stream);
-    return bgr ? launch_lanczos2_v2_sel<0x0123, 0, 4, 60, L2_THREADS, false, false, true> (d, st, v2, batch, n, stream)
-               : launch_lanczos2_v2_sel<0x0321, 0, 4, 60, L2_THREADS, false, false, true> (d, st, v2, batch, n, stream);
+      return bgr ? launch_lanczos2_v2_sel<0x0123, true, false, true> (d, st, v2, batch, n, stream)
+                 : launch_lanczos2_v2_sel<0x0321, true, false, true> (d, st, v2, batch, n, stream);
+    return bgr ? launch_lanczos2_v2_sel<0x0123, false, false, true> (d, st, v2, batch, n, stream)
+               : launch_lanczos2_v2_sel<0x0321, false, false, true> (d, st, v2, batch, n, stream);
   }
   if (d.yuv_out)                                  // the cross-family chain's first launch: scaled {255, Y, U, V} pixels, no matrix
-    return d.planar ? launch_lanczos2_v2_sel<-1, 0, 4, 60, L2_THREADS, true, true> (d, st, v2, batch, n, stream)
-                    : launch_lanczos2_v2_sel<-1, 0, 4, 60, L2_THREADS, false, true> (d, st, v2, batch, n, stream);
+    return d.planar ? launch_lanczos2_v2_sel<-1, true, true> (d, st, v2, batch, n, stream)
+                    : launch_lanczos2_v2_sel<-1, false, true> (d, st, v2, batch, n, stream);
   if (d.planar) {                                 // I420 / YV12 input
     switch (d.sel) {
-      case 0x0123u: return launch_lanczos2_v2_sel<0x0123, 0, 4, 60, L2_THREADS, true> (d, st, v2, batch, n, stream);
-      case 0x0321u: return launch_lanczos2_v2_sel<0x0321, 0, 4, 60, L2_THREADS, true> (d, st, v2, batch, n, stream);
-      default: return launch_lanczos2_v2_sel<-1, 0, 4, 60, L2_THREADS, true> (d, st, v2, batch, n, stream);
+      case 0x0123u: return launch_lanczos2_v2_sel<0x0123, true> (d, st, v2, batch, n, stream);
+      case 0x0321u: return launch_lanczos2_v2_sel<0x0321, true> (d, st, v2, batch, n, stream);
+      default: return launch_lanczos2_v2_sel<-1, true> (d, st, v2, batch, n, stream);
     }
   }
   switch (d.sel) {
-    // (prefetching the next item's loads was tried: slower)
-    case 0x0123u: return launch_lanczos2_v2_sel<0x0123, 0> (d, st, v2, batch, n, stream);   // BGRA / BGRx
-    case 0x0321u: return launch_lanczos2_v2_sel<0x0321, 0> (d, st, v2, batch, n, stream);   // RGBA / RGBx
-    default: return launch_lanczos2_v2_sel<-1, 0> (d, st, v2, batch, n, stream);
+    case 0x0123u: return launch_lanczos2_v2_sel<0x0123> (d, st, v2, batch, n, stream);   // BGRA / BGRx
+    case 0x0321u: return launch_lanczos2_v2_sel<0x0321> (d, st, v2, batch, n, stream);   // RGBA / RGBx
+    default: return launch_lanczos2_v2_sel<-1> (d, st, v2, batch, n, stream);
   }
 }
 
