@@ -493,7 +493,25 @@ struct ArsTile {
   const float4 *qtab;
 };
 
-// host side of the layout above; nch as computed at launch (ars_tile_geometry)
+// win and nch of a CTA that produces `no` consecutive outputs (qtab left null); nch does not depend on `no`
+static ArsTile ars_tile_geometry (const ArsPlan & p, int no)
+{
+  ArsTile t = ArsTile ();
+  // frames spanned by `no` outputs: ceil (no * in_step / out_step) + alignment + taps
+  const long long span = ((long long) no * p.in_step + p.out_step - 1) / p.out_step + 8 + p.n_taps;
+  t.win = (int) ((span + 3) & ~3LL);
+  const long long spread = ((long long) (ARS_RQ - 1) * p.in_step + p.out_step - 1) / p.out_step + 1;
+  t.nch = (int) ((spread + p.n_taps + 3 + 3) / 4 + 1);
+  return t;
+}
+
+// shared memory of a tile kernel CTA: the chunk-major taps of its no / RQ output groups, then its window of cb channels
+static size_t ars_tile_smem (const ArsTile & t, int no, int cb, int sample_bytes)
+{
+  return (size_t) (no / ARS_RQ) * t.nch * ARS_RQ * 4 * sizeof (float) + (size_t) t.win * cb * sample_bytes;
+}
+
+// host side of the layout above; nch from ars_tile_geometry
 static void ars_build_qtab (const ArsPlan & p, int nch, std::vector<float> * out)
 {
   const int RQ = 4;
@@ -1643,8 +1661,7 @@ static int ars_encode_window_map (ArsTensorMap *tm, const void *in, unsigned lon
     if (cudaGetDriverEntryPoint ("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) return nullptr;
     return (ars_encode_fn) f;
   } ();
-  static const bool off = getenv ("B200_ARS_NO_TENSORMAP") != nullptr;       // A/B knob: row-wise bulk copies only
-  if (!fn || off || !in || in_frames == 0 || win > 256 || cb > 256 || (((uintptr_t) in) & 15) || (channels & 3)) return 0;
+  if (!fn || !in || in_frames == 0 || win > 256 || cb > 256 || (((uintptr_t) in) & 15) || (channels & 3)) return 0;
   const cuuint64_t gdim[2] = {(cuuint64_t) channels, (cuuint64_t) in_frames};
   const cuuint64_t gstride[1] = {(cuuint64_t) channels * (cuuint64_t) elem_bytes};
   const cuuint32_t box[2] = {(cuuint32_t) cb, (cuuint32_t) win}, estr[2] = {1, 1};
@@ -1657,13 +1674,91 @@ static int ars_encode_window_map (ArsTensorMap *tm, const void *in, unsigned lon
 static int ars_encode_window_map (ArsTensorMap *, const void *, unsigned long long, int, int, int, int = 4) { return 0; }
 #endif
 
+// A/B and tuning switches of the resampler (README, environment knobs), read once when a handle is created
+struct ArsKnobs {
+  bool generic = false;          // B200_ARS_GENERIC: S16 runs ars_direct_kernel, F32 FULL ars_full_kernel
+  bool nopipe = false;           // B200_ARS_NOPIPE: no persistent pipeline
+  bool pipe_v1 = false;          // B200_ARS_PIPE_V1: the cp.async form of the F32 pipeline
+  bool no_tensormap = false;     // B200_ARS_NO_TENSORMAP: the pipelines' window copies row by row
+  int no = 32;                   // B200_ARS_NO: outputs per CTA of the F32 tile / generic kernel (4 .. 64, a power of two)
+  int cb = 0, cpt = 0;           // B200_ARS_CB (32, 64: at most this many channels per F32 tile CTA), B200_ARS_CPT (1, 4)
+  int grid = 0;                  // B200_ARS_GRID: at most this many persistent CTAs
+};
+
+static ArsKnobs ars_read_knobs ()
+{
+  ArsKnobs k;
+  k.generic = getenv ("B200_ARS_GENERIC") != nullptr;
+  k.nopipe = getenv ("B200_ARS_NOPIPE") != nullptr;
+  k.pipe_v1 = getenv ("B200_ARS_PIPE_V1") != nullptr;
+  k.no_tensormap = getenv ("B200_ARS_NO_TENSORMAP") != nullptr;
+  const char *no = getenv ("B200_ARS_NO"), *cb = getenv ("B200_ARS_CB"), *cpt = getenv ("B200_ARS_CPT"), *grid = getenv ("B200_ARS_GRID");
+  if (no && atoi (no) >= ARS_RQ && atoi (no) <= 64 && !(atoi (no) & (atoi (no) - 1))) k.no = atoi (no);   // s_rel/s_phase hold 64
+  if (cb && (atoi (cb) == 32 || atoi (cb) == 64)) k.cb = atoi (cb);
+  if (cpt && (atoi (cpt) == 1 || atoi (cpt) == 4)) k.cpt = atoi (cpt);
+  if (grid && atoi (grid) > 0) k.grid = atoi (grid);
+  return k;
+}
+
+// the kernel one b200_ars_process call runs (DESIGN.md §4.5)
+enum ArsKern { ARS_K_SMALL, ARS_K_DIRECT, ARS_K_INTERP, ARS_K_FULL, ARS_K_TILE, ARS_K_TILE_S16, ARS_K_PIPE, ARS_K_PIPE_V1, ARS_K_PIPE_S16 };
+
+struct ArsRoute {
+  int status = B200_OK;          // B200_ERR_UNSUPPORTED: ars_full_kernel's tap rows do not fit in shared memory
+  ArsKern kern = ARS_K_SMALL;
+  int no = 0;                    // outputs per CTA (tile, pipeline and generic kernels)
+  int cb = 0, cpt = 0;           // channels per CTA (ars_full_kernel: 32 x warps across channels), per thread (F32 tile)
+  ArsTile tile = ArsTile ();     // win and nch (tile and pipeline kernels)
+  size_t smem = 0;               // dynamic shared memory
+};
+
+// floats per staged tap row of ars_full_kernel: the taps shifted by up to 3, padded to a multiple of 4
+static int ars_row_pitch (const ArsPlan & p) { return (p.n_taps + 4 + 3) & ~3; }
+
+// smem_optin: the device's opt-in shared memory per block; aligned16: history, input and output are 16-byte aligned
+static ArsRoute ars_select_route (const ArsPlan & p, const ArsKnobs & k, int smem_optin, bool aligned16)
+{
+  if (p.small || p.copy) return {B200_OK, ARS_K_SMALL};
+  // the persistent pipelines: whole 128-channel blocks, 16-byte aligned streams, both stages in shared memory
+  const ArsTile pt = ars_tile_geometry (p, ARS_PIPE_NO);
+  const size_t pipe_smem = 2 * ars_tile_smem (pt, ARS_PIPE_NO, ARS_PIPE_CB, p.bps);
+  const bool pipe = (p.channels % ARS_PIPE_CB) == 0 && !k.generic && !k.nopipe && aligned16 && pipe_smem + 2048 <= (size_t) smem_optin;
+  if (p.fmt == ARS_S16 && p.full && !k.generic) {
+    if (pipe) return {B200_OK, ARS_K_PIPE_S16, ARS_PIPE_NO, ARS_PIPE_CB, 0, pt, pipe_smem};
+    // the tile kernel: the F32 tile geometry with 4-byte staged samples and taps
+    const int no = 32, cb = p.channels >= 128 ? 128 : 64;
+    const ArsTile t = ars_tile_geometry (p, no);
+    const size_t smem = ars_tile_smem (t, no, cb, 4);
+    if (p.channels >= 64 && smem <= (size_t) ARS_TILE_SMEM) return {B200_OK, ARS_K_TILE_S16, no, cb, 0, t, smem};
+  }
+  if (p.fmt != ARS_F32) return {B200_OK, ARS_K_DIRECT};
+  if (!p.full) return {B200_OK, ARS_K_INTERP};
+  const size_t row_bytes = (size_t) ars_row_pitch (p) * sizeof (float);
+  int no = k.no;                                                 // 32 by default: measured best for the tile kernel (3 CTAs / SM)
+  while (no > ARS_RQ && no * row_bytes > 96 * 1024) no >>= 1;
+  if (no * row_bytes > 160 * 1024) return {B200_ERR_UNSUPPORTED};
+  if (pipe) return {B200_OK, k.pipe_v1 ? ARS_K_PIPE_V1 : ARS_K_PIPE, ARS_PIPE_NO, ARS_PIPE_CB, 0, pt, pipe_smem};
+  int wcn = std::min ((p.channels + 31) / 32, 8);
+  while (8 % wcn) wcn++;                                         // 1, 2, 4 or 8 warps across channels
+  // the tile kernel when the CTA's input window fits in shared memory next to the chunk-major taps: 2 channels per thread
+  int cb = 32 * std::min (wcn, 4);
+  if (k.cb && k.cb < cb) cb = k.cb;
+  int cpt = cb >= 64 ? 2 : 1;
+  if (k.cpt == 1 || (k.cpt == 4 && cb >= 128)) cpt = k.cpt;
+  const ArsTile t = ars_tile_geometry (p, no);
+  const size_t smem = ars_tile_smem (t, no, cb, 4);
+  if (smem <= (size_t) ARS_TILE_SMEM && !k.generic) return {B200_OK, ARS_K_TILE, no, cb, cpt, t, smem};
+  return {B200_OK, ARS_K_FULL, no, 32 * wcn, 0, ArsTile (), no * row_bytes};
+}
+
 struct b200_ars {
   ArsPlan plan;
   int device = -1;
   b200_ars_config cfg;           // as created / last updated (b200_ars_update re-designs the filter from it)
+  ArsKnobs knobs;
+  int smem_optin = 0, sms = 0;   // the device's opt-in shared memory per block and its SM count
   float *d_phases = nullptr;
-  float *d_qtab = nullptr;       // chunk-major taps of every 4-output group (F32, FULL mode): see ArsTile::qtab
-  int qtab_nch = 0;
+  float *d_qtab = nullptr;       // chunk-major taps of every 4-output group (F32 FULL; S16 FULL in whole 128-channel blocks)
   float *d_proto = nullptr;      // interpolated mode: the oversampled prototype rows
   void *d_table_x = nullptr;     // other sample formats: phase taps (FULL) or prototype rows, in the samples' type
   float *d_hist[2] = {nullptr, nullptr};
@@ -1714,72 +1809,30 @@ static int ars_ensure_hist (b200_ars * h, int which, size_t frames, cudaStream_t
   return B200_OK;
 }
 
-// the plan's tables on the device (the current device is the handle's): phase taps or prototype rows, and for the F32 tile
-// kernels the pre-laid chunk-major rows
+// the plan's tables on the device (the current device is the handle's): phase taps or prototype rows, and for the tile and
+// pipeline kernels the pre-laid chunk-major rows
 static int ars_upload_tables (b200_ars * h)
 {
   int st;
+  const ArsPlan & q = h->plan;
   cudaFree (h->d_phases); cudaFree (h->d_qtab); cudaFree (h->d_proto); cudaFree (h->d_table_x);
-  h->d_phases = h->d_qtab = h->d_proto = nullptr; h->d_table_x = nullptr; h->qtab_nch = 0;
-  if (h->plan.fmt != ARS_F32) {
-    const std::vector<uint8_t> & t = h->plan.full ? h->plan.phases_x : h->plan.proto_x;
+  h->d_phases = h->d_qtab = h->d_proto = nullptr; h->d_table_x = nullptr;
+  if (q.fmt != ARS_F32) {
+    const std::vector<uint8_t> & t = q.full ? q.phases_x : q.proto_x;
     uint8_t *d = nullptr;
     st = upload (&d, t.data (), t.size ());
     h->d_table_x = d;
   } else
-    st = h->plan.full ? upload (&h->d_phases, h->plan.phases.data (), h->plan.phases.size ())
-                      : upload (&h->d_proto, h->plan.proto.data (), h->plan.proto.size ());
-  if (st == B200_OK && h->plan.fmt == ARS_S16 && h->plan.full && !h->plan.small && !h->plan.copy && (h->plan.channels % ARS_PIPE_CB) == 0 &&
-      h->plan.phases_x.size () == (size_t) h->plan.out_step * h->plan.n_taps * 2) {
-    // the pipelined S16 kernel's tap rows (32-bit ints in the F32 layout)
-    const ArsPlan & q = h->plan;
-    const long long spread = ((long long) (ARS_RQ - 1) * q.in_step + q.out_step - 1) / q.out_step + 1;
-    h->qtab_nch = (int) ((spread + q.n_taps + 3 + 3) / 4 + 1);
+    st = q.full ? upload (&h->d_phases, q.phases.data (), q.phases.size ()) : upload (&h->d_proto, q.proto.data (), q.proto.size ());
+  // tap rows of every (alignment, phase) group: F32 for the tile kernels and the pipeline, S16 (32-bit ints in the F32
+  // layout) for its pipeline; bounded by the FULL-mode threshold (bps * n_taps * out_rate < 1 MiB  =>  at most 16 x that)
+  if (st == B200_OK && q.full && !q.small && !q.copy && (q.fmt == ARS_F32 || (q.fmt == ARS_S16 && (q.channels % ARS_PIPE_CB) == 0))) {
     std::vector<float> tab;
-    ars_build_qtab_s16 (q, h->qtab_nch, &tab);
-    st = upload (&h->d_qtab, tab.data (), tab.size ());
-  }
-  if (st == B200_OK && h->plan.fmt == ARS_F32 && h->plan.full && !h->plan.small && !h->plan.copy) {
-    // tap rows of every (alignment, phase) group for the tile kernels; bounded by the FULL-mode threshold
-    // (bps * n_taps * out_rate < 1 MiB  =>  at most 16 x that in this layout)
-    const ArsPlan & q = h->plan;
-    const long long spread = ((long long) (ARS_RQ - 1) * q.in_step + q.out_step - 1) / q.out_step + 1;
-    h->qtab_nch = (int) ((spread + q.n_taps + 3 + 3) / 4 + 1);
-    std::vector<float> tab;
-    ars_build_qtab (q, h->qtab_nch, &tab);
+    if (q.fmt == ARS_F32) ars_build_qtab (q, ars_tile_geometry (q, 0).nch, &tab);
+    else ars_build_qtab_s16 (q, ars_tile_geometry (q, 0).nch, &tab);
     st = upload (&h->d_qtab, tab.data (), tab.size ());
   }
   return st;
-}
-
-// the pipelined S16 kernel (whole 128-channel blocks, 16-byte aligned streams); false: not applicable, take the tile kernel
-static bool ars_launch_pipe_s16 (b200_ars * h, ArsLaunch & L, size_t in_frames, size_t out_frames, cudaStream_t stream)
-{
-  const ArsPlan & p = h->plan;
-  ArsTile tp = ArsTile ();
-  const long long spread = ((long long) (ARS_RQ - 1) * p.in_step + p.out_step - 1) / p.out_step + 1;
-  tp.nch = (int) ((spread + p.n_taps + 3 + 3) / 4 + 1);
-  if (tp.nch != h->qtab_nch) return false;
-  const long long span = ((long long) ARS_PIPE_NO * p.in_step + p.out_step - 1) / p.out_step + 8 + p.n_taps;
-  tp.win = (int) ((span + 3) & ~3LL);
-  tp.qtab = (const float4 *) h->d_qtab;
-  const size_t smem_pipe = 2 * ((size_t) (ARS_PIPE_NO / ARS_RQ) * tp.nch * ARS_RQ * 4 * sizeof (float) + (size_t) tp.win * ARS_PIPE_CB * 2);
-  int optin = 0;
-  cudaDeviceGetAttribute (&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device);
-  if (smem_pipe + 2048 > (size_t) optin) return false;
-  static bool attr_done[16] = {false};
-  if (!attr_done[h->device & 15]) {
-    if (allow_max_dyn_smem (ars_pipe_kernel_s16) != B200_OK) return false;
-    attr_done[h->device & 15] = true;
-  }
-  L.no = ARS_PIPE_NO;
-  const int n_fb = (int) ((out_frames + ARS_PIPE_NO - 1) / ARS_PIPE_NO), n_cb = p.channels / ARS_PIPE_CB;
-  int grid = (int) std::min ((long long) n_fb * n_cb, (long long) sm_count (h->device));
-  { const char *e = getenv ("B200_ARS_GRID"); if (e && atoi (e) > 0) grid = std::min (grid, atoi (e)); }
-  ArsTensorMap tm = ArsTensorMap ();
-  const int use_tm = ars_encode_window_map (&tm, L.in, (unsigned long long) in_frames, p.channels, ARS_PIPE_CB, tp.win, 2);
-  ars_pipe_kernel_s16 <<<grid, ARS_PIPE_THREADS, smem_pipe, stream>>> (L, tp, n_fb, n_cb, tm, use_tm);
-  return true;
 }
 
 extern "C" {
@@ -1794,31 +1847,36 @@ int b200_ars_create (const b200_ars_config * cfg, int device, b200_ars ** handle
   int st = build_ars_plan (*cfg, &h->plan);
   if (st != B200_OK) { delete h; return st; }
   h->device = device;
+  h->knobs = ars_read_knobs ();
   h->samples_avail = h->plan.n_taps / 2 - 1;
   if (device >= 0) {
     int n = b200_device_count ();
     if (n <= 0) { delete h; return n < 0 ? n : B200_ERR_NO_DEVICE; }
     if (device >= n) { delete h; return B200_ERR_INVALID_ARG; }
     DeviceGuard g (device);
+    h->sms = sm_count (device);
     st = ars_upload_tables (h);
     if (st == B200_OK) st = ars_ensure_hist (h, 0, (size_t) h->plan.n_taps, nullptr);
     if (st == B200_OK) st = ars_ensure_hist (h, 1, (size_t) h->plan.n_taps, nullptr);
     if (st == B200_OK && cudaDeviceSynchronize () != cudaSuccess) st = B200_ERR_CUDA;   // clears done before any user stream
+    if (st == B200_OK && cudaDeviceGetAttribute (&h->smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device) != cudaSuccess)
+      st = B200_ERR_CUDA;
+    // the dynamic shared memory each kernel the route can pick may ask for; 0: the device's opt-in maximum
+    const struct { const void *fn; int bytes; } smem[] = {
+      {(const void *) ars_full_kernel, 160 * 1024}, {(const void *) ars_pipe_kernel, 0}, {(const void *) ars_pipe_kernel_v1, 0},
+      {(const void *) ars_pipe_kernel_s16, 0}, {(const void *) ars_tile_kernel<128, 4>, ARS_TILE_SMEM},
+      {(const void *) ars_tile_kernel<128, 2>, ARS_TILE_SMEM}, {(const void *) ars_tile_kernel<128, 1>, ARS_TILE_SMEM},
+      {(const void *) ars_tile_kernel<64, 2>, ARS_TILE_SMEM}, {(const void *) ars_tile_kernel<64, 1>, ARS_TILE_SMEM},
+      {(const void *) ars_tile_kernel<32, 1>, ARS_TILE_SMEM}, {(const void *) ars_tile_kernel_s16<128>, ARS_TILE_SMEM},
+      {(const void *) ars_tile_kernel_s16<64>, ARS_TILE_SMEM}};
+    for (size_t i = 0; st == B200_OK && i < sizeof (smem) / sizeof (smem[0]); i++) {
+      if (smem[i].bytes) cudaFuncSetAttribute (smem[i].fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem[i].bytes);
+      else st = allow_max_dyn_smem (smem[i].fn);
+    }
     if (st != B200_OK) {
       b200_ars_destroy (h);
       return st;
     }
-    cudaFuncSetAttribute (ars_full_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-    if ((st = allow_max_dyn_smem (ars_pipe_kernel)) != B200_OK) { b200_ars_destroy (h); return st; }
-    if ((st = allow_max_dyn_smem (ars_pipe_kernel_v1)) != B200_OK) { b200_ars_destroy (h); return st; }
-    cudaFuncSetAttribute (ars_tile_kernel<128, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, ARS_TILE_SMEM);
-    cudaFuncSetAttribute (ars_tile_kernel<128, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, ARS_TILE_SMEM);
-    cudaFuncSetAttribute (ars_tile_kernel<128, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, ARS_TILE_SMEM);
-    cudaFuncSetAttribute (ars_tile_kernel<64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, ARS_TILE_SMEM);
-    cudaFuncSetAttribute (ars_tile_kernel<64, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, ARS_TILE_SMEM);
-    cudaFuncSetAttribute (ars_tile_kernel<32, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, ARS_TILE_SMEM);
-    cudaFuncSetAttribute (ars_tile_kernel_s16<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, ARS_TILE_SMEM);
-    cudaFuncSetAttribute (ars_tile_kernel_s16<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, ARS_TILE_SMEM);
   }
   *handle = h;
   return B200_OK;
@@ -1973,139 +2031,78 @@ int b200_ars_process (b200_ars * h, const void *in_v, size_t in_frames, void *ou
   long long moved_from = 0;       // the absolute sample index the reference's buffers are shifted down by (macros.h:91-93)
   int new_phase = h->samp_phase;
   if (avail >= need && out_frames > 0) {
+    const bool aligned16 = ((((uintptr_t) h->d_hist[h->cur]) | ((uintptr_t) in_v) | ((uintptr_t) out_v)) & 15) == 0;
+    const ArsRoute r = ars_select_route (p, h->knobs, h->smem_optin, aligned16);
+    if (r.status != B200_OK) return r.status;
     ArsLaunch L;
-    L.hist = h->d_hist[h->cur]; L.in = in; L.out = out; L.phases = h->d_phases;
+    L.hist = h->d_hist[h->cur]; L.in = in; L.out = out;
+    L.phases = r.kern == ARS_K_TILE_S16 ? (const float *) h->d_table_x : h->d_phases;
     L.hist_frames = (long long) hist; L.avail = (long long) avail; L.out_frames = (long long) out_frames;
     L.channels = p.channels; L.n_taps = p.n_taps; L.out_step = p.out_step;
     L.samp_inc = p.samp_inc; L.samp_frac = p.samp_frac;
     L.samp_index = h->samp_index; L.samp_phase = h->samp_phase;
-    L.row_pitch = (p.n_taps + 4 + 3) & ~3;
-    L.wcn = (p.channels + 31) / 32; if (L.wcn > 8) L.wcn = 8;
-    while (8 % L.wcn) L.wcn++;                                   // 1, 2, 4 or 8 warps across channels
-    bool s16_tiled = false;           // ... or the small-method kernel: launched already
-    if (p.small || p.copy) {
-      ArsLaunchX X;
-      X.hist = h->d_hist[h->cur]; X.in = in_v; X.out = out_v;
-      X.table = p.fmt == ARS_F32 ? (const void *) h->d_phases : (const void *) h->d_table_x;
-      X.hist_frames = (long long) hist; X.avail = (long long) avail; X.out_frames = (long long) out_frames;
-      X.channels = p.channels; X.n_taps = p.n_taps; X.out_step = p.out_step;
-      X.samp_inc = p.samp_inc; X.samp_frac = p.samp_frac; X.samp_index = h->samp_index; X.samp_phase = h->samp_phase;
-      X.full = 1; X.oversample = 1;
-      const int nearest = p.small == B200_ARS_METHOD_NEAREST || p.copy;
-      const dim3 grid ((unsigned) ((out_frames + ARS_THREADS / 32 - 1) / (ARS_THREADS / 32)), (unsigned) ((p.channels + 31) / 32));
-      if (p.fmt == ARS_S16) ars_small_kernel<ARS_S16> <<<grid, ARS_THREADS, 0, stream>>> (X, nearest);
-      else if (p.fmt == ARS_S32) ars_small_kernel<ARS_S32> <<<grid, ARS_THREADS, 0, stream>>> (X, nearest);
-      else if (p.fmt == ARS_F64) ars_small_kernel<ARS_F64> <<<grid, ARS_THREADS, 0, stream>>> (X, nearest);
-      else ars_small_kernel<ARS_F32> <<<grid, ARS_THREADS, 0, stream>>> (X, nearest);
-      s16_tiled = true;
-    } else if (p.fmt == ARS_S16 && p.full && h->d_qtab && (p.channels % ARS_PIPE_CB) == 0 && !getenv ("B200_ARS_GENERIC") &&
-        !getenv ("B200_ARS_NOPIPE") && ((((uintptr_t) L.hist) | ((uintptr_t) L.in) | ((uintptr_t) L.out)) & 15) == 0 &&
-        ars_launch_pipe_s16 (h, L, in_frames, out_frames, stream)) {
-      s16_tiled = true;
-    } else if (p.fmt == ARS_S16 && p.full && p.channels >= 64 && !getenv ("B200_ARS_GENERIC")) {
-      // tiled S16 kernel: same tile geometry as the F32 one (4-byte staged samples and taps)
-      const int cb = p.channels >= 128 ? 128 : 64, no = 32;
-      ArsTile tl = ArsTile ();
-      const long long span = ((long long) no * p.in_step + p.out_step - 1) / p.out_step + 8 + p.n_taps;
-      tl.win = (int) ((span + 3) & ~3LL);
-      const long long spread = ((long long) (ARS_RQ - 1) * p.in_step + p.out_step - 1) / p.out_step + 1;
-      tl.nch = (int) ((spread + p.n_taps + 3 + 3) / 4 + 1);
-      const size_t smem_tile = ((size_t) (no / ARS_RQ) * tl.nch * ARS_RQ * 4 + (size_t) tl.win * cb) * sizeof (float);
-      if (smem_tile <= (size_t) ARS_TILE_SMEM) {
-        L.no = no; L.row_pitch = 0; L.wcn = 1;
-        L.phases = (const float *) h->d_table_x;
-        const dim3 grid ((unsigned) ((out_frames + no - 1) / no), (unsigned) ((p.channels + cb - 1) / cb));
-        if (cb == 128) ars_tile_kernel_s16<128> <<<grid, ARS_THREADS, smem_tile, stream>>> (L, tl);
-        else ars_tile_kernel_s16<64> <<<grid, ARS_THREADS, smem_tile, stream>>> (L, tl);
-        s16_tiled = true;
-      }
-    }
-    if (s16_tiled) {
-    } else if (p.fmt != ARS_F32) {
-      ArsLaunchX X;
-      X.hist = h->d_hist[h->cur]; X.in = in_v; X.out = out_v; X.table = h->d_table_x;
-      X.hist_frames = (long long) hist; X.avail = (long long) avail; X.out_frames = (long long) out_frames;
-      X.channels = p.channels; X.n_taps = p.n_taps; X.out_step = p.out_step;
-      X.samp_inc = p.samp_inc; X.samp_frac = p.samp_frac; X.samp_index = h->samp_index; X.samp_phase = h->samp_phase;
-      X.full = p.full ? 1 : 0; X.oversample = p.oversample;
-      const dim3 grid ((unsigned) ((out_frames + ARS_THREADS / 32 - 1) / (ARS_THREADS / 32)), (unsigned) ((p.channels + 31) / 32));
-      const bool lin = p.linear && !p.full;
-      if (p.fmt == ARS_S16) {
-        if (lin) ars_direct_kernel<ARS_S16, true> <<<grid, ARS_THREADS, 0, stream>>> (X);
-        else ars_direct_kernel<ARS_S16, false> <<<grid, ARS_THREADS, 0, stream>>> (X);
-      } else if (p.fmt == ARS_S32) {
-        if (lin) ars_direct_kernel<ARS_S32, true> <<<grid, ARS_THREADS, 0, stream>>> (X);
-        else ars_direct_kernel<ARS_S32, false> <<<grid, ARS_THREADS, 0, stream>>> (X);
-      } else {
-        if (lin) ars_direct_kernel<ARS_F64, true> <<<grid, ARS_THREADS, 0, stream>>> (X);
-        else ars_direct_kernel<ARS_F64, false> <<<grid, ARS_THREADS, 0, stream>>> (X);
-      }
-    } else if (!p.full) {
-      L.no = 0; L.row_pitch = 0; L.wcn = 1;
-      const dim3 grid ((unsigned) ((out_frames + ARS_THREADS / 32 - 1) / (ARS_THREADS / 32)), (unsigned) ((p.channels + 31) / 32));
-      if (p.linear) ars_interp_kernel<true> <<<grid, ARS_THREADS, 0, stream>>> (L, h->d_proto, p.oversample);
-      else ars_interp_kernel<false> <<<grid, ARS_THREADS, 0, stream>>> (L, h->d_proto, p.oversample);
-    } else {
-    const char *env_no = getenv ("B200_ARS_NO"), *env_cpt = getenv ("B200_ARS_CPT");
-    int no = env_no ? atoi (env_no) : 32;                        // measured best for the non-persistent tile kernel (3 CTAs / SM)
-    if (no < ARS_RQ || no > 64 || (no & (no - 1))) no = 32;      // s_rel/s_phase hold 64 outputs
-    while (no > ARS_RQ && (size_t) no * L.row_pitch * sizeof (float) > 96 * 1024) no >>= 1;
-    if ((size_t) no * L.row_pitch * sizeof (float) > 160 * 1024) return B200_ERR_UNSUPPORTED;
-    L.no = no;
-    // fast path when the CTA's input window fits in shared memory next to the chunk-major taps
-    ArsTile tl = ArsTile ();
-    int cb = 32 * (L.wcn > 4 ? 4 : L.wcn);
-    { const char *e = getenv ("B200_ARS_CB"); if (e && (atoi (e) == 64 || atoi (e) == 32) && atoi (e) < cb) cb = atoi (e); }   // tuning knob
-    // channels per thread: 2 (B200_ARS_CPT overrides)
-    int cpt = cb >= 64 ? 2 : 1;
-    if (env_cpt && (atoi (env_cpt) == 1 || (atoi (env_cpt) == 4 && cb >= 128))) cpt = atoi (env_cpt);
-    {
-      // frames spanned by `no` outputs: ceil (no * in_step / out_step) + alignment + taps
-      const long long span = ((long long) no * p.in_step + p.out_step - 1) / p.out_step + 8 + p.n_taps;
-      tl.win = (int) ((span + 3) & ~3LL);
-      const long long spread = ((long long) (ARS_RQ - 1) * p.in_step + p.out_step - 1) / p.out_step + 1;
-      tl.nch = (int) ((spread + p.n_taps + 3 + 3) / 4 + 1);
-      tl.qtab = (const float4 *) h->d_qtab;
-    }
-    const size_t smem_tile = ((size_t) (no / ARS_RQ) * tl.nch * ARS_RQ * 4 + (size_t) tl.win * cb) * sizeof (float);
-    // the persistent pipeline: whole 128-channel blocks, 16-byte aligned streams, both buffers in shared memory
-    bool piped = false;
-    if (h->d_qtab && tl.nch == h->qtab_nch && (p.channels % ARS_PIPE_CB) == 0 && !getenv ("B200_ARS_GENERIC") && !getenv ("B200_ARS_NOPIPE") &&
-        ((((uintptr_t) L.hist) | ((uintptr_t) L.in) | ((uintptr_t) L.out)) & 15) == 0) {
-      ArsTile tp = tl;
-      const long long span = ((long long) ARS_PIPE_NO * p.in_step + p.out_step - 1) / p.out_step + 8 + p.n_taps;
-      tp.win = (int) ((span + 3) & ~3LL);
-      const size_t smem_pipe = 2 * ((size_t) (ARS_PIPE_NO / ARS_RQ) * tp.nch * ARS_RQ * 4 + (size_t) tp.win * ARS_PIPE_CB) * sizeof (float);
-      int optin = 0;
-      cudaDeviceGetAttribute (&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device);
-      if (smem_pipe + 2048 <= (size_t) optin) {
-        L.no = ARS_PIPE_NO;
+    L.no = r.no; L.wcn = r.cb / 32; L.row_pitch = ars_row_pitch (p);
+    ArsLaunchX X;
+    X.hist = L.hist; X.in = in_v; X.out = out_v;
+    X.table = p.fmt == ARS_F32 ? (const void *) h->d_phases : (const void *) h->d_table_x;
+    X.hist_frames = L.hist_frames; X.avail = L.avail; X.out_frames = L.out_frames;
+    X.channels = p.channels; X.n_taps = p.n_taps; X.out_step = p.out_step;
+    X.samp_inc = p.samp_inc; X.samp_frac = p.samp_frac; X.samp_index = h->samp_index; X.samp_phase = h->samp_phase;
+    X.full = p.full ? 1 : 0; X.oversample = p.oversample;
+    ArsTile T = r.tile;
+    T.qtab = (const float4 *) h->d_qtab;
+    // one warp per output frame x 32 channels; the tile and generic kernels: no outputs x cb channels per CTA
+    const dim3 warps ((unsigned) ((out_frames + ARS_THREADS / 32 - 1) / (ARS_THREADS / 32)), (unsigned) ((p.channels + 31) / 32));
+    auto tiles = [&] { return dim3 ((unsigned) ((out_frames + r.no - 1) / r.no), (unsigned) ((p.channels + r.cb - 1) / r.cb)); };
+    const int nearest = p.small == B200_ARS_METHOD_NEAREST || p.copy;
+    const bool lin = p.linear && !p.full;
+    switch (r.kern) {
+      case ARS_K_SMALL:
+        if (p.fmt == ARS_S16) ars_small_kernel<ARS_S16> <<<warps, ARS_THREADS, 0, stream>>> (X, nearest);
+        else if (p.fmt == ARS_S32) ars_small_kernel<ARS_S32> <<<warps, ARS_THREADS, 0, stream>>> (X, nearest);
+        else if (p.fmt == ARS_F64) ars_small_kernel<ARS_F64> <<<warps, ARS_THREADS, 0, stream>>> (X, nearest);
+        else ars_small_kernel<ARS_F32> <<<warps, ARS_THREADS, 0, stream>>> (X, nearest);
+        break;
+      case ARS_K_DIRECT:
+        if (p.fmt == ARS_S16 && lin) ars_direct_kernel<ARS_S16, true> <<<warps, ARS_THREADS, 0, stream>>> (X);
+        else if (p.fmt == ARS_S16) ars_direct_kernel<ARS_S16, false> <<<warps, ARS_THREADS, 0, stream>>> (X);
+        else if (p.fmt == ARS_S32 && lin) ars_direct_kernel<ARS_S32, true> <<<warps, ARS_THREADS, 0, stream>>> (X);
+        else if (p.fmt == ARS_S32) ars_direct_kernel<ARS_S32, false> <<<warps, ARS_THREADS, 0, stream>>> (X);
+        else if (lin) ars_direct_kernel<ARS_F64, true> <<<warps, ARS_THREADS, 0, stream>>> (X);
+        else ars_direct_kernel<ARS_F64, false> <<<warps, ARS_THREADS, 0, stream>>> (X);
+        break;
+      case ARS_K_INTERP:
+        if (p.linear) ars_interp_kernel<true> <<<warps, ARS_THREADS, 0, stream>>> (L, h->d_proto, p.oversample);
+        else ars_interp_kernel<false> <<<warps, ARS_THREADS, 0, stream>>> (L, h->d_proto, p.oversample);
+        break;
+      case ARS_K_FULL:
+        ars_full_kernel <<<tiles (), ARS_THREADS, r.smem, stream>>> (L);
+        break;
+      case ARS_K_TILE:
+        if (r.cb == 128 && r.cpt == 4) ars_tile_kernel<128, 4> <<<tiles (), ARS_THREADS, r.smem, stream>>> (L, T);
+        else if (r.cb == 128 && r.cpt == 2) ars_tile_kernel<128, 2> <<<tiles (), ARS_THREADS, r.smem, stream>>> (L, T);
+        else if (r.cb == 128) ars_tile_kernel<128, 1> <<<tiles (), ARS_THREADS, r.smem, stream>>> (L, T);
+        else if (r.cb == 64 && r.cpt == 2) ars_tile_kernel<64, 2> <<<tiles (), ARS_THREADS, r.smem, stream>>> (L, T);
+        else if (r.cb == 64) ars_tile_kernel<64, 1> <<<tiles (), ARS_THREADS, r.smem, stream>>> (L, T);
+        else ars_tile_kernel<32, 1> <<<tiles (), ARS_THREADS, r.smem, stream>>> (L, T);
+        break;
+      case ARS_K_TILE_S16:
+        if (r.cb == 128) ars_tile_kernel_s16<128> <<<tiles (), ARS_THREADS, r.smem, stream>>> (L, T);
+        else ars_tile_kernel_s16<64> <<<tiles (), ARS_THREADS, r.smem, stream>>> (L, T);
+        break;
+      case ARS_K_PIPE: case ARS_K_PIPE_V1: case ARS_K_PIPE_S16: {
+        // persistent CTAs walk the (64-output, 128-channel) tiles; the input's tensor map changes with every buffer
         const int n_fb = (int) ((out_frames + ARS_PIPE_NO - 1) / ARS_PIPE_NO), n_cb = p.channels / ARS_PIPE_CB;
-        int grid = (int) std::min ((long long) n_fb * n_cb, (long long) sm_count (h->device));
-        { const char *e = getenv ("B200_ARS_GRID"); if (e && atoi (e) > 0) grid = std::min (grid, atoi (e)); }   // tuning / test knob: persistent CTAs
-        static const bool v1 = getenv ("B200_ARS_PIPE_V1") != nullptr;   // A/B knob: the cp.async form
-        if (v1) ars_pipe_kernel_v1 <<<grid, ARS_PIPE_THREADS, smem_pipe, stream>>> (L, tp, n_fb, n_cb);
-        else {
-          ArsTensorMap tm = ArsTensorMap ();
-          const int use_tm = ars_encode_window_map (&tm, L.in, (unsigned long long) in_frames, p.channels, ARS_PIPE_CB, tp.win);
-          ars_pipe_kernel <<<grid, ARS_PIPE_THREADS, smem_pipe, stream>>> (L, tp, n_fb, n_cb, tm, use_tm);
-        }
-        piped = true;
+        int grid = (int) std::min ((long long) n_fb * n_cb, (long long) h->sms);
+        if (h->knobs.grid) grid = std::min (grid, h->knobs.grid);
+        ArsTensorMap tm = ArsTensorMap ();
+        const int use_tm = r.kern != ARS_K_PIPE_V1 && !h->knobs.no_tensormap &&
+            ars_encode_window_map (&tm, in_v, (unsigned long long) in_frames, p.channels, ARS_PIPE_CB, T.win, p.bps);
+        if (r.kern == ARS_K_PIPE) ars_pipe_kernel <<<grid, ARS_PIPE_THREADS, r.smem, stream>>> (L, T, n_fb, n_cb, tm, use_tm);
+        else if (r.kern == ARS_K_PIPE_S16) ars_pipe_kernel_s16 <<<grid, ARS_PIPE_THREADS, r.smem, stream>>> (L, T, n_fb, n_cb, tm, use_tm);
+        else ars_pipe_kernel_v1 <<<grid, ARS_PIPE_THREADS, r.smem, stream>>> (L, T, n_fb, n_cb);
+        break;
       }
-    }
-    if (piped) {
-    } else if (smem_tile <= (size_t) ARS_TILE_SMEM && h->d_qtab && tl.nch == h->qtab_nch && !getenv ("B200_ARS_GENERIC")) {
-      const dim3 grid ((unsigned) ((out_frames + no - 1) / no), (unsigned) ((p.channels + cb - 1) / cb));
-      if (cb == 128 && cpt == 4) ars_tile_kernel<128, 4> <<<grid, ARS_THREADS, smem_tile, stream>>> (L, tl);
-      else if (cb == 128 && cpt == 2) ars_tile_kernel<128, 2> <<<grid, ARS_THREADS, smem_tile, stream>>> (L, tl);
-      else if (cb == 128) ars_tile_kernel<128, 1> <<<grid, ARS_THREADS, smem_tile, stream>>> (L, tl);
-      else if (cb == 64 && cpt == 2) ars_tile_kernel<64, 2> <<<grid, ARS_THREADS, smem_tile, stream>>> (L, tl);
-      else if (cb == 64) ars_tile_kernel<64, 1> <<<grid, ARS_THREADS, smem_tile, stream>>> (L, tl);
-      else ars_tile_kernel<32, 1> <<<grid, ARS_THREADS, smem_tile, stream>>> (L, tl);
-    } else {
-      const dim3 grid ((unsigned) ((out_frames + no - 1) / no), (unsigned) ((p.channels + 32 * L.wcn - 1) / (32 * L.wcn)));
-      ars_full_kernel <<<grid, ARS_THREADS, (size_t) no * L.row_pitch * sizeof (float), stream>>> (L);
-    }
     }
     B200_CUDA_TRY (cudaGetLastError ());
     // state after out_frames outputs (closed form of the stepping loop)
@@ -2118,10 +2115,10 @@ int b200_ars_process (b200_ars * h, const void *in_v, size_t in_frames, void *ou
     h->samp_phase = new_phase;
   }
   // history: what the reference keeps in its per-channel buffers (macros.h:91-93, :1790-1804)
-  size_t first = 0, keep = avail;
+  size_t keep = avail;
   if (consumed > 0) {
-    if (avail > consumed) { first = consumed; keep = avail - consumed; }
-    else { first = avail; keep = 0; h->skip = (int) (consumed - avail); }
+    if (avail > consumed) keep = avail - consumed;
+    else { keep = 0; h->skip = (int) (consumed - avail); }
   }
   const int nxt = h->cur ^ 1;
   int st = ars_ensure_hist (h, nxt, keep, stream);
@@ -2131,7 +2128,6 @@ int b200_ars_process (b200_ars * h, const void *in_v, size_t in_frames, void *ou
   // decimating: the next window starts beyond the data), and then the last `initial` of the kept samples are not the
   // stream's tail but whatever the shift left in place: the frames at those same buffer positions.  Part 1 = frames
   // [moved_from, ...) -> position 0, part 2 = frames [n1, keep) staying where they were (empty without a skip).
-  (void) first;
   const size_t n1 = (long long) avail > moved_from ? std::min (keep, (size_t) ((long long) avail - moved_from)) : 0;
   auto copy_hist = [&] (size_t dst_frame, long long from, size_t count) {
     if (!count) return;

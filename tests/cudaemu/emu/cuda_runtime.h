@@ -46,8 +46,9 @@ extern thread_local dim3 blockDim, gridDim;
 namespace b200emu {
 extern uint8_t *dyn_smem;         // the launch's dynamic shared memory: a heap block of exactly the requested size
 void barrier ();
-// runs body once per thread of every block of the grid; in record-only mode it appends the kernel's name to the launch
-// log instead.  `name` is the kernel as the launch site spells it; `fn` resolves it to its instantiation.
+// runs body once per thread of every block of the grid; in record-only mode it appends the kernel's name (at level 2 with
+// grid, block and shared-memory bytes) to the launch log instead.  `name` is the kernel as the launch site spells it; `fn`
+// resolves it to its instantiation.
 void launch (dim3 grid, dim3 block, size_t smem_bytes, const std::function<void ()> & body, const char *name, const void *fn);
 }
 

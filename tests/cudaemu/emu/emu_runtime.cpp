@@ -131,7 +131,7 @@ static void *thread_main (void *arg)
 }
 
 static std::string g_log;                      // kernels launched in record-only mode, one per line
-static bool g_record_only = false;
+static int g_record_only = 0;                  // 0: run launches; 1: log the kernel; 2: the kernel and its launch configuration
 
 // the instantiation `fn` points at, without namespace, return type and parameters ("vcs_generic_kernel<false>"); the
 // launch site's spelling where the symbol is not exported (a function pointer's variable name, e.g. "fn")
@@ -159,6 +159,10 @@ void launch (dim3 grid, dim3 block, size_t smem_bytes, const std::function<void 
 {
   if (g_record_only) {
     g_log += kernel_label (name, fn);
+    if (g_record_only >= 2)
+      g_log += " grid=" + std::to_string (grid.x) + "," + std::to_string (grid.y) + "," + std::to_string (grid.z) + " block=" +
+               std::to_string (block.x) + "," + std::to_string (block.y) + "," + std::to_string (block.z) + " smem=" +
+               std::to_string (smem_bytes);
     g_log += '\n';
     return;
   }
@@ -192,7 +196,8 @@ extern "C" {
 // the kernels launched since the last clear, one name per line (valid until the next launch or clear)
 const char *b200emu_launch_log () { return b200emu::g_log.c_str (); }
 void b200emu_clear_launch_log () { b200emu::g_log.clear (); }
-// on: launches are logged and no block runs (route tests); off (the default): launches run and are not logged
-void b200emu_set_record_only (int on) { b200emu::g_record_only = on != 0; }
+// 1: launches are logged by kernel and no block runs (route tests); 2: the same, each line followed by
+// " grid=x,y,z block=x,y,z smem=bytes"; 0 (the default): launches run and are not logged
+void b200emu_set_record_only (int level) { b200emu::g_record_only = level; }
 
 }
