@@ -11,6 +11,7 @@
 // HBM traffic per frame = every covered source pixel once + the destination once
 // (the reference moves bg write + per pad src read + dst read + dst write).
 #include "common.h"
+#include "video_format.h"
 
 #include <string.h>
 #include <algorithm>
@@ -359,18 +360,13 @@ int b200_comp_create (int out_format, int width, int height, int device, b200_co
   if (!handle) return B200_ERR_INVALID_ARG;
   *handle = nullptr;
   if (width < 1 || height < 1 || width > 32767 || height > 32767) return B200_ERR_INVALID_ARG;
+  // packed RGB with alpha: the alpha byte's shift in the little-endian pixel word (blend.h:55-66: rgba uses the bgra
+  // kernels, abgr the argb ones); planar / semi-planar YUV: -1, b200_comp_blend_yuv
+  const b200::VideoFormatDesc *d = b200::video_format (out_format);
   int shift;
-  switch (out_format) {          // blend.h:55-66: rgba uses the bgra kernels, abgr the argb ones
-    case B200_VIDEO_FORMAT_BGRA: case B200_VIDEO_FORMAT_RGBA: shift = 24; break;
-    case B200_VIDEO_FORMAT_ARGB: case B200_VIDEO_FORMAT_ABGR: shift = 0; break;
-    case B200_VIDEO_FORMAT_I420: case B200_VIDEO_FORMAT_YV12: case B200_VIDEO_FORMAT_NV12: case B200_VIDEO_FORMAT_NV21:
-    case B200_VIDEO_FORMAT_Y444: case B200_VIDEO_FORMAT_Y42B:
-    case B200_VIDEO_FORMAT_I420_10LE: case B200_VIDEO_FORMAT_I420_12LE: case B200_VIDEO_FORMAT_I422_10LE:
-    case B200_VIDEO_FORMAT_I422_12LE: case B200_VIDEO_FORMAT_Y444_10LE: case B200_VIDEO_FORMAT_Y444_12LE:
-    case B200_VIDEO_FORMAT_Y444_16LE:
-      shift = -1; break;                                           // planar / semi-planar YUV output: b200_comp_blend_yuv
-    default: return B200_ERR_UNSUPPORTED;
-  }
+  if (d && d->family == b200::FAMILY_RGB && d->alpha) shift = 8 * d->pos[0];
+  else if (d && (d->family == b200::FAMILY_YUV420 || d->family == b200::FAMILY_NV || d->family == b200::FAMILY_YUV_PLANAR)) shift = -1;
+  else return B200_ERR_UNSUPPORTED;
   if (device >= 0) {
     int n = b200_device_count ();
     if (n <= 0) return n < 0 ? n : B200_ERR_NO_DEVICE;
@@ -464,25 +460,12 @@ int b200_comp_blend_yuv (b200_comp * h, void *dst, const b200_video_info * di, i
   if (h->device < 0) return B200_ERR_NO_DEVICE;
   DeviceGuard g (h->device);
   if (!g.ok) return B200_ERR_CUDA;
-  // the format's PLANAR_YUV_BLEND / NV_YUV_BLEND instantiation (blend.c:591-646, :1386): chroma sub-sampling shifts, the
-  // x_round / y_round of the position, bytes per sample and depth
-  bool semi = false;
-  int ws = 1, hs = 1, xr = 2, yr = 2, es = 1, nbits = 8;
-  switch (h->format) {
-    case B200_VIDEO_FORMAT_NV12: case B200_VIDEO_FORMAT_NV21: semi = true; break;
-    case B200_VIDEO_FORMAT_I420: case B200_VIDEO_FORMAT_YV12: break;
-    case B200_VIDEO_FORMAT_Y444: ws = hs = 0; xr = yr = 1; break;
-    case B200_VIDEO_FORMAT_Y42B: hs = 0; yr = 1; break;
-    case B200_VIDEO_FORMAT_I420_10LE: es = 2; nbits = 10; break;
-    case B200_VIDEO_FORMAT_I420_12LE: es = 2; nbits = 12; break;
-    case B200_VIDEO_FORMAT_I422_10LE: es = 2; nbits = 10; hs = 0; yr = 1; break;
-    case B200_VIDEO_FORMAT_I422_12LE: es = 2; nbits = 12; hs = 0; yr = 1; break;
-    case B200_VIDEO_FORMAT_Y444_10LE: es = 2; nbits = 10; ws = hs = 0; xr = yr = 1; break;
-    case B200_VIDEO_FORMAT_Y444_12LE: es = 2; nbits = 12; ws = hs = 0; xr = yr = 1; break;
-    case B200_VIDEO_FORMAT_Y444_16LE: es = 2; nbits = 16; ws = hs = 0; xr = yr = 1; break;
-    default: return B200_ERR_STATE;
-  }
-  const int W = h->width, H = h->height, n_planes = semi ? 2 : 3;
+  // the format's PLANAR_YUV_BLEND / NV_YUV_BLEND instantiation (blend.c:591-646, :1386): chroma sub-sampling shifts,
+  // bytes per sample and depth from the format table; the position rounds up to the chroma grid (x_round / y_round)
+  const b200::VideoFormatDesc & d = *b200::video_format (h->format);
+  const bool semi = d.family == b200::FAMILY_NV;
+  const int ws = d.wsub, hs = d.hsub, xr = 1 << ws, yr = 1 << hs, es = d.bytes, nbits = d.depth;
+  const int W = h->width, H = h->height, n_planes = d.n_planes;
   auto sub = [] (int v, int sh) { return -((-v) >> sh); };         // GST_VIDEO_FORMAT_INFO_SCALE_WIDTH / _HEIGHT (round up)
   CompYuvParams P;
   memset (&P, 0, sizeof (P));

@@ -6,6 +6,7 @@
 // (gst-plugins-bad/gst-libs/gst/cuda/gstcudaconverter.cpp:1911).
 #include "common.h"
 #include "vcs_plan.h"
+#include "video_format.h"
 #include "vcs_device.h"
 #include "vcs_kernels.cuh"
 #include "vcs_lanczos2.cuh"
@@ -22,6 +23,7 @@
 #include "vcs_yuy2_420.cuh"
 
 #include <string.h>
+#include <algorithm>
 #include <new>
 #include <vector>
 
@@ -488,9 +490,9 @@ int prepare_device (b200_vcs * h)
     if (p.yuy2_420) {
       Yuy2Dev & y = h->yuy2;
       memset (&y, 0, sizeof (y));
-      const bool uyvy = p.in.format == B200_VIDEO_FORMAT_UYVY;
+      const bool y_odd = video_format (p.in.format)->pair_y == 1;   // UYVY: luma in the odd bytes
       y.w = p.in.width; y.h = p.in.height; y.sstride = p.in.stride[0]; y.soff = p.in.offset[0];
-      y.sel_y = uyvy ? 0x7531 : 0x6420; y.sel_c = uyvy ? 0x6420 : 0x7531;
+      y.sel_y = y_odd ? 0x7531 : 0x6420; y.sel_c = y_odd ? 0x6420 : 0x7531;
       y.svec = ((y.sstride | y.soff) & 15) == 0 ? 2 : (((y.sstride | y.soff) & 3) == 0 ? 1 : 0);
       y.stride_y = q.stride_y; y.stride_u = q.stride_u; y.stride_v = q.stride_v;
       y.off_y = q.off_y; y.off_u = q.off_u; y.off_v = q.off_v;
@@ -568,114 +570,41 @@ void b200_vcs_config_init (b200_vcs_config * cfg)
   cfg->border_argb = 0xff000000u; cfg->fill_border = 1;   // DEFAULT_OPT_FILL_BORDER / _BORDER_ARGB, video-converter.c:778, :782
 }
 
+// video-info.c:882-894 (packed), :997-1063 (8-bit planar and semi-planar), :1142-1188 (10 / 12 / 16 bits); RGBP / BGRP
+// are laid out like Y444 (:1030-1041)
 int b200_video_info_set_format (b200_video_info * info, int format, int width, int height)
 {
   if (!info || width < 1 || height < 1) return B200_ERR_INVALID_ARG;
   memset (info, 0, sizeof (*info));
   info->format = format; info->width = width; info->height = height;
-  switch (format) {
-    case B200_VIDEO_FORMAT_NV12: case B200_VIDEO_FORMAT_NV21:
-      // video-info.c:1053-1063
-      info->stride[0] = (width + 3) & ~3; info->stride[1] = info->stride[0];
-      info->offset[0] = 0; info->offset[1] = (uint64_t) info->stride[0] * ((height + 1) & ~1);
-      info->color_matrix = height > 576 ? B200_COLOR_MATRIX_BT709 : B200_COLOR_MATRIX_BT601;
-      info->color_range = B200_COLOR_RANGE_16_235;
-      info->chroma_site = height > 576 ? B200_CHROMA_SITE_H_COSITED : B200_CHROMA_SITE_NONE;
-      return B200_OK;
-    case B200_VIDEO_FORMAT_I420: case B200_VIDEO_FORMAT_YV12:
-      // video-info.c:997-1009 (YV12: same layout, the format description swaps planes 1 and 2)
-      info->stride[0] = (width + 3) & ~3;
-      info->stride[1] = info->stride[2] = ((((width + 1) & ~1) / 2) + 3) & ~3;
-      info->offset[0] = 0; info->offset[1] = (uint64_t) info->stride[0] * ((height + 1) & ~1);
-      info->offset[2] = info->offset[1] + (uint64_t) info->stride[1] * (((height + 1) & ~1) / 2);
-      info->color_matrix = height > 576 ? B200_COLOR_MATRIX_BT709 : B200_COLOR_MATRIX_BT601;
-      info->color_range = B200_COLOR_RANGE_16_235;
-      info->chroma_site = height > 576 ? B200_CHROMA_SITE_H_COSITED : B200_CHROMA_SITE_NONE;
-      return B200_OK;
-    case B200_VIDEO_FORMAT_YUY2: case B200_VIDEO_FORMAT_UYVY: case B200_VIDEO_FORMAT_YVYU:
-    case B200_VIDEO_FORMAT_Y42B: case B200_VIDEO_FORMAT_Y444:
-      if (format == B200_VIDEO_FORMAT_Y42B) {                      // video-info.c:1020-1029
-        info->stride[0] = (width + 3) & ~3;
-        info->stride[1] = info->stride[2] = ((width + 7) & ~7) / 2;
-        info->offset[1] = (uint64_t) info->stride[0] * height;
-        info->offset[2] = info->offset[1] + (uint64_t) info->stride[1] * height;
-      } else if (format == B200_VIDEO_FORMAT_Y444) {               // :1030-1041
-        info->stride[0] = info->stride[1] = info->stride[2] = (width + 3) & ~3;
-        info->offset[1] = (uint64_t) info->stride[0] * height;
-        info->offset[2] = info->offset[1] * 2;
-      } else info->stride[0] = (width * 2 + 3) & ~3;               // :882-889
-      info->color_matrix = height > 576 ? B200_COLOR_MATRIX_BT709 : B200_COLOR_MATRIX_BT601;
-      info->color_range = B200_COLOR_RANGE_16_235;
-      info->chroma_site = height > 576 ? B200_CHROMA_SITE_H_COSITED : B200_CHROMA_SITE_NONE;
-      return B200_OK;
-    case B200_VIDEO_FORMAT_RGBx: case B200_VIDEO_FORMAT_BGRx: case B200_VIDEO_FORMAT_xRGB:
-    case B200_VIDEO_FORMAT_xBGR: case B200_VIDEO_FORMAT_RGBA: case B200_VIDEO_FORMAT_BGRA:
-    case B200_VIDEO_FORMAT_ARGB: case B200_VIDEO_FORMAT_ABGR:
-      info->stride[0] = width * 4;      // video-info.c:890-894
-      info->color_matrix = B200_COLOR_MATRIX_RGB; info->color_range = B200_COLOR_RANGE_0_255;
-      return B200_OK;
-    case B200_VIDEO_FORMAT_RGBP: case B200_VIDEO_FORMAT_BGRP:        // video-info.c:1030-1041 (the Y444 case)
-      info->stride[0] = info->stride[1] = info->stride[2] = (width + 3) & ~3;
-      info->offset[1] = (uint64_t) info->stride[0] * height;
-      info->offset[2] = info->offset[1] * 2;
-      info->color_matrix = B200_COLOR_MATRIX_RGB; info->color_range = B200_COLOR_RANGE_0_255;
-      return B200_OK;
-    case B200_VIDEO_FORMAT_I420_10LE: case B200_VIDEO_FORMAT_I420_12LE:       // video-info.c:1142-1156
-    case B200_VIDEO_FORMAT_I422_10LE: case B200_VIDEO_FORMAT_I422_12LE: {     // :1157-1169
-      const bool is420 = format == B200_VIDEO_FORMAT_I420_10LE || format == B200_VIDEO_FORMAT_I420_12LE;
-      const int hh = (height + 1) & ~1;
-      info->stride[0] = (width * 2 + 3) & ~3;
-      info->stride[1] = info->stride[2] = (width + 3) & ~3;
-      info->offset[1] = (uint64_t) info->stride[0] * hh;
-      info->offset[2] = info->offset[1] + (uint64_t) info->stride[1] * (is420 ? hh / 2 : hh);
-      info->color_matrix = height > 576 ? B200_COLOR_MATRIX_BT709 : B200_COLOR_MATRIX_BT601;
-      info->color_range = B200_COLOR_RANGE_16_235;
-      info->chroma_site = height > 576 ? B200_CHROMA_SITE_H_COSITED : B200_CHROMA_SITE_NONE;
-      return B200_OK;
+  const VideoFormatDesc *d = video_format (format);
+  if (!d) return B200_ERR_UNSUPPORTED;
+  if (d->n_planes == 1) {
+    info->stride[0] = (width * (d->family == FAMILY_RGB ? 4 : 2) + 3) & ~3;
+  } else {
+    const int cw = (width + (1 << d->wsub) - 1) >> d->wsub, rows = luma_rows (*d, height);
+    info->stride[0] = (width * d->bytes + 3) & ~3;
+    info->stride[1] = d->family == FAMILY_NV ? info->stride[0] : (cw * d->bytes + 3) & ~3;
+    info->offset[1] = (uint64_t) info->stride[0] * rows;
+    if (d->n_planes == 3) {
+      info->stride[2] = info->stride[1];
+      info->offset[2] = info->offset[1] + (uint64_t) info->stride[1] * (rows >> d->hsub);
     }
-    case B200_VIDEO_FORMAT_Y444_10LE: case B200_VIDEO_FORMAT_Y444_12LE: case B200_VIDEO_FORMAT_Y444_16LE:   // :1170-1188
-      info->stride[0] = info->stride[1] = info->stride[2] = (width * 2 + 3) & ~3;
-      info->offset[1] = (uint64_t) info->stride[0] * height;
-      info->offset[2] = info->offset[1] * 2;
-      info->color_matrix = height > 576 ? B200_COLOR_MATRIX_BT709 : B200_COLOR_MATRIX_BT601;
-      info->color_range = B200_COLOR_RANGE_16_235;
-      info->chroma_site = height > 576 ? B200_CHROMA_SITE_H_COSITED : B200_CHROMA_SITE_NONE;
-      return B200_OK;
-    default:
-      return B200_ERR_UNSUPPORTED;
   }
+  fill_colorimetry (info, *d, height);
+  return B200_OK;
 }
 
 size_t b200_video_info_size (const b200_video_info * info)
 {
   if (!info) return 0;
-  switch (info->format) {
-    case B200_VIDEO_FORMAT_NV12: case B200_VIDEO_FORMAT_NV21:
-      return (size_t) info->offset[1] + (size_t) info->stride[1] * (((info->height + 1) & ~1) / 2);
-    case B200_VIDEO_FORMAT_I420: case B200_VIDEO_FORMAT_YV12: {
-      const size_t ch = (size_t) (((info->height + 1) & ~1) / 2);
-      const size_t e1 = (size_t) info->offset[1] + (size_t) info->stride[1] * ch;
-      const size_t e2 = (size_t) info->offset[2] + (size_t) info->stride[2] * ch;
-      return e1 > e2 ? e1 : e2;
-    }
-    case B200_VIDEO_FORMAT_Y42B: case B200_VIDEO_FORMAT_Y444:
-    case B200_VIDEO_FORMAT_Y444_10LE: case B200_VIDEO_FORMAT_Y444_12LE: case B200_VIDEO_FORMAT_Y444_16LE:
-      return (size_t) info->offset[2] + (size_t) info->stride[2] * info->height;
-    case B200_VIDEO_FORMAT_I420_10LE: case B200_VIDEO_FORMAT_I420_12LE:
-      return (size_t) info->offset[2] + (size_t) info->stride[2] * (((info->height + 1) & ~1) / 2);
-    case B200_VIDEO_FORMAT_I422_10LE: case B200_VIDEO_FORMAT_I422_12LE:
-      return (size_t) info->offset[2] + (size_t) info->stride[2] * ((info->height + 1) & ~1);
-    case B200_VIDEO_FORMAT_RGBP: case B200_VIDEO_FORMAT_BGRP: {       // three full planes in any order
-      size_t end = 0;
-      for (int k = 0; k < 3; k++) {
-        const size_t e = (size_t) info->offset[k] + (size_t) info->stride[k] * info->height;
-        if (e > end) end = e;
-      }
-      return end;
-    }
-    default:
-      return (size_t) info->offset[0] + (size_t) info->stride[0] * info->height;
-  }
+  const VideoFormatDesc *d = video_format (info->format);
+  if (!d || d->n_planes == 1) return (size_t) info->offset[0] + (size_t) info->stride[0] * info->height;
+  const int rows = luma_rows (*d, info->height);
+  auto end = [&] (int k) { return (size_t) info->offset[k] + (size_t) info->stride[k] * (k ? rows >> d->hsub : rows); };
+  if (d->family == FAMILY_RGBP) return std::max ({end (0), end (1), end (2)});      // three full planes in any order
+  if (d->family == FAMILY_YUV420 && d->bytes == 1) return std::max (end (1), end (2));   // either chroma plane last
+  return end (d->n_planes - 1);
 }
 
 int b200_vcs_create (const b200_video_info * in, const b200_video_info * out,
@@ -695,13 +624,12 @@ int b200_vcs_create (const b200_video_info * in, const b200_video_info * out,
     const b200_video_info & f = q.frame_out;
     BorderDev & b = h->border;
     memset (&b, 0, sizeof (b));
-    const bool rgb = f.format >= B200_VIDEO_FORMAT_RGBx && f.format <= B200_VIDEO_FORMAT_ABGR;
-    const bool planar = f.format == B200_VIDEO_FORMAT_I420 || f.format == B200_VIDEO_FORMAT_YV12;
+    const VideoFormatDesc & d = *video_format (f.format);
     if (q.rgbp_out) {                                               // pack_RGBP of the border line: each plane its own byte
       b.n_planes = 3;
       for (int k = 0; k < 3; k++)
         b.pl[k] = BorderPlane {f.offset[k], f.stride[k], f.width, f.height, 1, q.dest[0], q.dest[1], q.dest[2], q.dest[3], (unsigned) q.border_px[k]};
-    } else if (rgb) {
+    } else if (d.family == FAMILY_RGB) {
       b.n_planes = 1;
       b.pl[0] = BorderPlane {f.offset[0], f.stride[0], f.width, f.height, 4, q.dest[0], q.dest[1], q.dest[2], q.dest[3],
         (unsigned) q.border_px[0] | ((unsigned) q.border_px[1] << 8) | ((unsigned) q.border_px[2] << 16) | ((unsigned) q.border_px[3] << 24)};
@@ -709,15 +637,14 @@ int b200_vcs_create (const b200_video_info * in, const b200_video_info * out,
       const int cx = (q.dest[0] + 1) / 2, cy = (q.dest[1] + 1) / 2, cw = (q.dest[2] + 1) / 2, chh = (q.dest[3] + 1) / 2;
       const int CW = (f.width + 1) / 2, CH = (f.height + 1) / 2;
       b.pl[0] = BorderPlane {f.offset[0], f.stride[0], f.width, f.height, 1, q.dest[0], q.dest[1], q.dest[2], q.dest[3], (unsigned) q.border_yuv[0]};
-      if (planar) {
-        const int pu = f.format == B200_VIDEO_FORMAT_YV12 ? 2 : 1, pv = 3 - pu;
-        b.n_planes = 3;
+      const int pu = d.plane_u, pv = d.plane_v;
+      b.n_planes = d.n_planes;
+      if (d.family == FAMILY_YUV420) {
         b.pl[1] = BorderPlane {f.offset[pu], f.stride[pu], CW, CH, 1, cx, cy, cw, chh, (unsigned) q.border_yuv[1]};
         b.pl[2] = BorderPlane {f.offset[pv], f.stride[pv], CW, CH, 1, cx, cy, cw, chh, (unsigned) q.border_yuv[2]};
-      } else {
+      } else {                                                      // one interleaved pair: U at byte u_index
         const unsigned u = (unsigned) q.border_yuv[1], v = (unsigned) q.border_yuv[2];
-        b.n_planes = 2;
-        b.pl[1] = BorderPlane {f.offset[1], f.stride[1], CW, CH, 2, cx, cy, cw, chh, f.format == B200_VIDEO_FORMAT_NV21 ? (v | (u << 8)) : (u | (v << 8))};
+        b.pl[1] = BorderPlane {f.offset[pu], f.stride[pu], CW, CH, 2, cx, cy, cw, chh, u << (8 * d.u_index) | v << (8 - 8 * d.u_index)};
       }
     }
   }

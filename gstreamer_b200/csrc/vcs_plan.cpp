@@ -10,6 +10,7 @@
 //   chroma pairing             video-converter.c:571-617, :2991-3021; video-chroma.c:959-1036
 //   element option mapping     gst/videoconvertscale/gstvideoconvertscale.c:991-1087
 #include "vcs_plan.h"
+#include "video_format.h"
 
 #include <math.h>
 #include <stdio.h>
@@ -557,21 +558,18 @@ void validate_fast_geometry (VcsPlan * p)
 }
 
 // setup_scale (video-converter.c:8092-8245) for planar in/out (4:2:0 same family; Y42B / Y444 -> I420 / YV12): what each output plane does
-int build_planes (VcsPlan * p, const FilterSpec & f)
+int build_planes (VcsPlan * p, const VideoFormatDesc & fi, const VideoFormatDesc & fo, const FilterSpec & f)
 {
-  const bool semi = p->out.format == B200_VIDEO_FORMAT_NV12 || p->out.format == B200_VIDEO_FORMAT_NV21;
+  const bool semi = fo.family == FAMILY_NV;
   const int iw = p->in.width, ih = p->in.height, ow = p->out.width, oh = p->out.height;
   p->planes_mode = true;
-  p->n_planes = semi ? 2 : 3;
+  p->n_planes = fo.n_planes;
   for (int i = 0; i < p->n_planes; i++) {
     PlanePlan & q = p->planes[i];
     q = PlanePlan ();
-    // exactly one side YV12: U and V planes swap (the source plane is the one holding the same component)
-    q.src_plane = (!semi && i > 0 && (p->in.format == B200_VIDEO_FORMAT_YV12) != (p->out.format == B200_VIDEO_FORMAT_YV12)) ? 3 - i : i;
-    // chroma plane size of the input: 4:2:0 halves both directions, Y42B the width only, Y444 neither
-    const int in_wsub = p->in.format == B200_VIDEO_FORMAT_Y444 ? 0 : 1;
-    const int in_hsub = (p->in.format == B200_VIDEO_FORMAT_Y444 || p->in.format == B200_VIDEO_FORMAT_Y42B) ? 0 : 1;
-    q.iw = i ? (iw + in_wsub) >> in_wsub : iw; q.ih = i ? (ih + in_hsub) >> in_hsub : ih;
+    // the source plane is the input's plane holding the same component (I420 <-> YV12 swap U and V)
+    q.src_plane = i == 0 ? 0 : (i == fo.plane_u ? fi.plane_u : fi.plane_v);
+    q.iw = i ? (iw + fi.wsub) >> fi.wsub : iw; q.ih = i ? (ih + fi.hsub) >> fi.hsub : ih;
     q.ow = i ? (ow + 1) / 2 : ow; q.oh = i ? (oh + 1) / 2 : oh;
     q.ne = (semi && i == 1) ? 2 : 1;
     if (p->in.stride[q.src_plane] < q.iw * q.ne || p->out.stride[i] < q.ow * q.ne) return B200_ERR_INVALID_ARG;
@@ -602,6 +600,15 @@ int build_planes (VcsPlan * p, const FilterSpec & f)
 
 }  // namespace
 
+// nibble k of the result: the input byte of the component that `out` stores at byte (or plane) k, for the components
+// `first` .. B (0 = A, 1 = R, 2 = G, 3 = B; pos[] of the format table)
+static unsigned byte_map (const VideoFormatDesc & in, const VideoFormatDesc & out, int first)
+{
+  unsigned m = 0;
+  for (int c = first; c < 4; c++) m |= (unsigned) in.pos[c] << (4 * out.pos[c]);
+  return m;
+}
+
 // packed RGB -> 4:2:0 (the encoder-feeding direction): no table row in the reference, its generic chain: unpack to
 // ARGB, the scalers that shrink, the RGB -> YUV table matrix, the scalers that grow, chroma down-sampling (RGB has no
 // sub-sampling, so only the down side exists and it exists at every size: video-converter.c:2850-2895), 4:2:0 pack.
@@ -610,18 +617,7 @@ int build_planes (VcsPlan * p, const FilterSpec & f)
 // convert_scale_planes rows (video-converter.c:8879-8896): 4-byte pixels through gst_video_scaler_2d with the element's
 // method, the stepping 2-tap horizontal scaler (video_scale_h_2tap_4u8), every byte - alpha or padding included - a
 // channel.  vcs_planes_kernel with ne = 4.
-// memory byte index of the A (or padding), R, G, B component of a packed 4-byte format
-static void rgb_component_bytes (int format, int pos[4])
-{
-  switch (format) {
-    case B200_VIDEO_FORMAT_BGRA: case B200_VIDEO_FORMAT_BGRx: pos[0] = 3; pos[1] = 2; pos[2] = 1; pos[3] = 0; break;
-    case B200_VIDEO_FORMAT_RGBA: case B200_VIDEO_FORMAT_RGBx: pos[0] = 3; pos[1] = 0; pos[2] = 1; pos[3] = 2; break;
-    case B200_VIDEO_FORMAT_ABGR: case B200_VIDEO_FORMAT_xBGR: pos[0] = 0; pos[1] = 3; pos[2] = 2; pos[3] = 1; break;
-    default: pos[0] = 0; pos[1] = 1; pos[2] = 2; pos[3] = 3; break;          // ARGB / xRGB
-  }
-}
-
-static int build_rgb_same_plan (VcsPlan * p)
+static int build_rgb_same_plan (VcsPlan * p, const VideoFormatDesc & fi, const VideoFormatDesc & fo)
 {
   const b200_video_info *in = &p->in, *out = &p->out;
   const int iw = in->width, ih = in->height, ow = out->width, oh = out->height;
@@ -638,11 +634,7 @@ static int build_rgb_same_plan (VcsPlan * p)
   // and in where each byte lands; a format's padding byte travels as alpha, like in the reference's unpack
   const bool cross = in->format != out->format;
   if (cross) {
-    int pi[4], po[4];
-    rgb_component_bytes (in->format, pi);
-    rgb_component_bytes (out->format, po);
-    unsigned swz = 0;
-    for (int comp = 0; comp < 4; comp++) swz |= (unsigned) pi[comp] << (4 * po[comp]);
+    const unsigned swz = byte_map (fi, fo, 0);
     q.swz = swz == 0x3210u ? 0u : swz;
   }
   if (iw == ow && ih == oh) { q.mode = PM_COPY; return B200_OK; }
@@ -655,11 +647,6 @@ static int build_rgb_same_plan (VcsPlan * p)
   return B200_OK;
 }
 
-static bool is_rgbp (int format)
-{
-  return format == B200_VIDEO_FORMAT_RGBP || format == B200_VIDEO_FORMAT_BGRP;
-}
-
 // every plane of a planar RGB output holds at least a row of the frame
 static bool rgbp_strides_ok (const b200_video_info & o)
 {
@@ -670,16 +657,13 @@ static bool rgbp_strides_ok (const b200_video_info & o)
 // the scalers in chain_scale's pass order (like another packed RGB order, build_rgb_same_plan), pack_RGBP / pack_BGRP
 // (video-format.c:7496-7536: R, G, B bytes, alpha dropped).  Every byte is an independent channel, so the 4-byte
 // pixels are scaled in the input's own byte order and the de-interleave picks the components.
-static int build_rgb_rgbp_plan (VcsPlan * p)
+static int build_rgb_rgbp_plan (VcsPlan * p, const VideoFormatDesc & fi, const VideoFormatDesc & fo)
 {
   const b200_video_info *in = &p->in, *out = &p->out;
   const int iw = in->width, ih = in->height, ow = out->width, oh = out->height;
   if (in->stride[0] < iw * 4 || !rgbp_strides_ok (*out)) return B200_ERR_INVALID_ARG;
-  int pi[4];
-  rgb_component_bytes (in->format, pi);
-  const bool bgr = out->format == B200_VIDEO_FORMAT_BGRP;
   p->rgbp_out = true;
-  p->deint_sel = (unsigned) pi[bgr ? 3 : 1] | (unsigned) pi[2] << 4 | (unsigned) pi[bgr ? 1 : 3] << 8;
+  p->deint_sel = byte_map (fi, fo, 1);
   const FilterSpec f = filter_from_method (p->cfg);
   p->planes_mode = true;
   p->n_planes = 1;
@@ -695,42 +679,33 @@ static int build_rgb_rgbp_plan (VcsPlan * p)
   return B200_OK;
 }
 
-static int build_rgb_in_plan (VcsPlan * p)
+// 4:2:0 output of the chain: the planes and the byte of U / V the chroma pack writes; false when a plane's stride is
+// shorter than its row
+static bool set_420_output (VcsPlan * p, const VideoFormatDesc & fo)
+{
+  const b200_video_info *out = &p->out;
+  const int ocw = (out->width + 1) / 2;
+  const bool semi = fo.family == FAMILY_NV;
+  if (out->stride[0] < out->width || out->stride[1] < (semi ? 2 * ocw : ocw) || (!semi && out->stride[2] < ocw))
+    return false;
+  p->out_plane_u = fo.plane_u; p->out_plane_v = fo.plane_v;
+  p->out_cstep = semi ? 2 : 1; p->out_u_index = fo.u_index;
+  return true;
+}
+
+static int build_rgb_in_plan (VcsPlan * p, const VideoFormatDesc & fi, const VideoFormatDesc & fo)
 {
   const b200_video_info *in = &p->in, *out = &p->out;
-  if (out->format >= B200_VIDEO_FORMAT_RGBx && out->format <= B200_VIDEO_FORMAT_ABGR) return build_rgb_same_plan (p);
-  if (is_rgbp (out->format)) return build_rgb_rgbp_plan (p);
-  const bool out_pl = out->format == B200_VIDEO_FORMAT_I420 || out->format == B200_VIDEO_FORMAT_YV12;
-  const bool out_semi = out->format == B200_VIDEO_FORMAT_NV12 || out->format == B200_VIDEO_FORMAT_NV21;
-  if (!out_pl && !out_semi) return B200_ERR_UNSUPPORTED;
   if (in->stride[0] < in->width * 4 || (in->stride[0] & 3) || (in->offset[0] & 3)) return B200_ERR_INVALID_ARG;
-  const int ocw = (out->width + 1) / 2;
-  if (out->stride[0] < out->width) return B200_ERR_INVALID_ARG;
-  if (out_pl) {
-    if (out->stride[1] < ocw || out->stride[2] < ocw) return B200_ERR_INVALID_ARG;
-    p->out_plane_u = out->format == B200_VIDEO_FORMAT_YV12 ? 2 : 1;
-    p->out_plane_v = 3 - p->out_plane_u;
-    p->out_cstep = 1; p->out_u_index = 0;
-  } else {
-    if (out->stride[1] < 2 * ocw) return B200_ERR_INVALID_ARG;
-    p->out_plane_u = p->out_plane_v = 1;
-    p->out_cstep = 2; p->out_u_index = out->format == B200_VIDEO_FORMAT_NV21 ? 1 : 0;
-  }
-  // caps defaults of the output size where the caller left them open (the fixation forwards only primaries and
-  // transfer across an RGB/YUV change, gstvideoconvertscale.c:1394-1408)
-  if (p->in.color_range == 0) p->in.color_range = B200_COLOR_RANGE_0_255;
-  if (p->out.color_matrix == 0) p->out.color_matrix = out->height > 576 ? B200_COLOR_MATRIX_BT709 : B200_COLOR_MATRIX_BT601;
-  if (p->out.color_range == 0) p->out.color_range = B200_COLOR_RANGE_16_235;
-  if (p->out.chroma_site == 0) p->out.chroma_site = out->height > 576 ? B200_CHROMA_SITE_H_COSITED : B200_CHROMA_SITE_NONE;
+  if (!set_420_output (p, fo)) return B200_ERR_INVALID_ARG;
+  // caps defaults where the caller left them open: the output takes those of its size (the fixation forwards only
+  // primaries and transfer across an RGB/YUV change, gstvideoconvertscale.c:1394-1408)
+  fill_colorimetry (&p->in, fi, in->height);
+  fill_colorimetry (&p->out, fo, out->height);
   int st = colour_matrix_rgb2yuv (p);
   if (st != B200_OK) return st;
   p->rgb_in = p->yuv_out = true;
-  switch (in->format) {                 // source byte of R, G, B, A (nibbles 0..3)
-    case B200_VIDEO_FORMAT_BGRA: case B200_VIDEO_FORMAT_BGRx: p->in_sel = 0x3012; break;
-    case B200_VIDEO_FORMAT_RGBA: case B200_VIDEO_FORMAT_RGBx: p->in_sel = 0x3210; break;
-    case B200_VIDEO_FORMAT_ABGR: case B200_VIDEO_FORMAT_xBGR: p->in_sel = 0x0123; break;
-    default: p->in_sel = 0x0321; break;                            // ARGB / xRGB
-  }
+  p->in_sel = fi.pos[1] | fi.pos[2] << 4 | fi.pos[3] << 8 | fi.pos[0] << 12;   // source byte of R, G, B, A
   { uint8_t s[4] = {0, 1, 2, 3}; memcpy (p->byte_sel, s, 4); }
   p->planar = false; p->u_index = 0; p->h_cosited = false; p->v_pairs = false; p->chroma_nearest = false;
   FilterSpec f = filter_from_method (p->cfg);
@@ -748,27 +723,62 @@ static int build_rgb_in_plan (VcsPlan * p)
   return B200_OK;
 }
 
+// what the converter builds for a format pair
+enum PlanClass : int {
+  PC_PLANES,                            // plane scaling (convert_scale_planes table rows): build_planes
+  PC_RGB_RGB,                           // packed RGB -> packed RGB: build_rgb_same_plan
+  PC_RGB_RGBP,                          // packed RGB -> RGBP / BGRP: build_rgb_rgbp_plan
+  PC_RGB_420,                           // packed RGB -> 4:2:0: build_rgb_in_plan
+  PC_420_RGB,                           // 4:2:0 -> packed RGB, RGBP / BGRP: build_chain_plan from here on
+  PC_420_CHAIN,                         // 4:2:0 -> the other 4:2:0 family
+  PC_422_RGB,                           // 4:2:2 / 4:4:4 -> packed RGB, RGBP / BGRP
+  PC_422_420,                           // 4:2:2 / 4:4:4 -> 4:2:0 through the chain
+};
+
+// the 8-bit 4:2:0 formats: the converter's YUV outputs
+static bool is_420 (const VideoFormatDesc * d)
+{
+  return d && d->bytes == 1 && (d->family == FAMILY_YUV420 || d->family == FAMILY_NV);
+}
+
+// (input, output) -> the plan class, or B200_ERR_UNSUPPORTED for a pair the converter does not take
+static int classify (const VideoFormatDesc * fi, const VideoFormatDesc * fo)
+{
+  if (!fi || fi->bytes != 1 || fi->family == FAMILY_RGBP) return B200_ERR_UNSUPPORTED;
+  const bool out_rgb = fo && (fo->family == FAMILY_RGB || fo->family == FAMILY_RGBP);
+  switch (fi->family) {
+    case FAMILY_RGB:
+      if (out_rgb) return fo->family == FAMILY_RGB ? PC_RGB_RGB : PC_RGB_RGBP;
+      return is_420 (fo) ? PC_RGB_420 : B200_ERR_UNSUPPORTED;
+    case FAMILY_YUV420: case FAMILY_NV:
+      // the reference has plane-scaling table rows for NV12 -> NV12, NV21 -> NV21 and I420 / YV12 -> I420 / YV12
+      // (video-converter.c:8722-8760); the other 4:2:0 pairs have none: the generic chain, closed by chain_downsample
+      // (video-converter.c:2018-2032) and the 4:2:0 pack functions
+      if (is_420 (fo))
+        return fi->family == fo->family && (fi->family == FAMILY_YUV420 || fi->format == fo->format) ? PC_PLANES : PC_420_CHAIN;
+      return out_rgb ? PC_420_RGB : B200_ERR_UNSUPPORTED;
+    default:
+      // planar 4:2:2 / 4:4:4 -> planar 4:2:0 are plane-scaling table rows like I420 -> I420 (video-converter.c:8607-8628);
+      // -> semi-planar 4:2:0 and every packed 4:2:2 pair run the chain
+      if (fi->family == FAMILY_YUV_PLANAR && is_420 (fo) && fo->family == FAMILY_YUV420) return PC_PLANES;
+      if (out_rgb) return PC_422_RGB;
+      return is_420 (fo) ? PC_422_420 : B200_ERR_UNSUPPORTED;
+  }
+}
+
 static int build_inner_plan (const b200_video_info * in, const b200_video_info * out,
     const b200_vcs_config * cfg, VcsPlan * p, bool resample_forced);
 
 // border pixel of setup_borderline (video-converter.c:2189-2258): packed RGB outputs take border_argb's bytes in the
 // format's order; YUV outputs convert it with the un-scaled (no x256) rint'ed RGB -> YCbCr matrix of the OUTPUT
 // colorimetry and hand-added 16 / 128 / 128 offsets
-static int border_colour (VcsPlan * p, const b200_video_info & fo, uint32_t argb_word)
+static int border_colour (VcsPlan * p, const VideoFormatDesc & fo, uint32_t argb_word)
 {
   const int a = argb_word >> 24, r = (argb_word >> 16) & 0xff, g = (argb_word >> 8) & 0xff, b = argb_word & 0xff;
-  const bool rgb = (fo.format >= B200_VIDEO_FORMAT_RGBx && fo.format <= B200_VIDEO_FORMAT_ABGR) || is_rgbp (fo.format);
-  if (rgb) {
+  if (fo.family == FAMILY_RGB || fo.family == FAMILY_RGBP) {
     // RGBP / BGRP: border_px[k] is the byte of plane k (pack_RGBP / pack_BGRP of the border line)
-    const uint8_t comp[4] = {(uint8_t) a, (uint8_t) r, (uint8_t) g, (uint8_t) b};
-    uint8_t sel[4];
-    switch (fo.format) {
-      case B200_VIDEO_FORMAT_BGRA: case B200_VIDEO_FORMAT_BGRx: case B200_VIDEO_FORMAT_BGRP: { uint8_t s_[4] = {3, 2, 1, 0}; memcpy (sel, s_, 4); break; }
-      case B200_VIDEO_FORMAT_RGBA: case B200_VIDEO_FORMAT_RGBx: case B200_VIDEO_FORMAT_RGBP: { uint8_t s_[4] = {1, 2, 3, 0}; memcpy (sel, s_, 4); break; }
-      case B200_VIDEO_FORMAT_ABGR: case B200_VIDEO_FORMAT_xBGR: { uint8_t s_[4] = {0, 3, 2, 1}; memcpy (sel, s_, 4); break; }
-      default: { uint8_t s_[4] = {0, 1, 2, 3}; memcpy (sel, s_, 4); break; }
-    }
-    for (int i = 0; i < 4; i++) p->border_px[i] = comp[sel[i]];
+    const int comp[4] = {a, r, g, b};
+    for (int c = 0; c < 4; c++) p->border_px[fo.pos[c]] = (uint8_t) comp[c];
     return B200_OK;
   }
   // the plan's `out` carries the resolved output colorimetry (the input's for 4:2:0 -> 4:2:0, the caps defaults of
@@ -818,38 +828,26 @@ int build_vcs_plan (const b200_video_info * in, const b200_video_info * out,
   // GST_VIDEO_CONVERTER_OPT_DEST_* (video-converter.c:2333-2362): the chain scales into the rectangle; for sub-sampled
   // outputs its origin is rounded down to the chroma grid; it is clipped to the frame
   if (out->width < 1 || out->height < 1 || out->width > 32767 || out->height > 32767) return B200_ERR_INVALID_ARG;
-  const bool yuv = out->format == B200_VIDEO_FORMAT_I420 || out->format == B200_VIDEO_FORMAT_YV12 ||
-      out->format == B200_VIDEO_FORMAT_NV12 || out->format == B200_VIDEO_FORMAT_NV21;
-  const bool planar = out->format == B200_VIDEO_FORMAT_I420 || out->format == B200_VIDEO_FORMAT_YV12;
+  const VideoFormatDesc *fi = video_format (in->format), *fo = video_format (out->format);
+  const bool yuv = is_420 (fo);
   int dx = cfg->dest_x, dy = cfg->dest_y, dw = cfg->dest_width, dh = cfg->dest_height;
   if (yuv) { dx &= ~1; dy &= ~1; }
   if (dx < 0 || dy < 0 || dw < 0 || dh < 0) return B200_ERR_INVALID_ARG;
   if (dw > out->width - dx) dw = out->width - dx;
   if (dh > out->height - dy) dh = out->height - dy;
   if (dw < 1 || dh < 1) return B200_ERR_INVALID_ARG;               // an empty rectangle: degenerate in the reference too
-  if (is_rgbp (out->format) && !rgbp_strides_ok (*out)) return B200_ERR_INVALID_ARG;
+  if (fo && fo->family == FAMILY_RGBP && !rgbp_strides_ok (*out)) return B200_ERR_INVALID_ARG;
   b200_video_info inner = *out;
   inner.width = dw; inner.height = dh;
-  if (is_rgbp (out->format)) {                                     // no sub-sampling: every plane at (dx, dy)
-    for (int k = 0; k < 3; k++) inner.offset[k] += (uint64_t) dy * out->stride[k] + (uint64_t) dx;
-  } else if (!yuv) inner.offset[0] += (uint64_t) dy * out->stride[0] + (uint64_t) dx * 4;
-  else {
-    inner.offset[0] += (uint64_t) dy * out->stride[0] + (uint64_t) dx;
-    if (planar) {
-      inner.offset[1] += (uint64_t) (dy / 2) * out->stride[1] + (uint64_t) (dx / 2);
-      inner.offset[2] += (uint64_t) (dy / 2) * out->stride[2] + (uint64_t) (dx / 2);
-    } else inner.offset[1] += (uint64_t) (dy / 2) * out->stride[1] + (uint64_t) dx;
+  for (int k = 0; fo && k < fo->n_planes; k++) {                  // each plane's origin on its own sampling grid
+    const int px = fo->family == FAMILY_RGB ? 4 : (fo->family == FAMILY_NV && k ? 2 : 1);
+    inner.offset[k] += (uint64_t) (k ? dy >> fo->hsub : dy) * out->stride[k] + (uint64_t) (k ? dx >> fo->wsub : dx) * px;
   }
-  // colorimetry defaults belong to the whole frame, not to the rectangle
-  const bool in_rgb = in->format >= B200_VIDEO_FORMAT_RGBx && in->format <= B200_VIDEO_FORMAT_ABGR;
-  if (yuv && in_rgb) {
-    if (inner.color_matrix == 0) inner.color_matrix = out->height > 576 ? B200_COLOR_MATRIX_BT709 : B200_COLOR_MATRIX_BT601;
-    if (inner.color_range == 0) inner.color_range = B200_COLOR_RANGE_16_235;
-    if (inner.chroma_site == 0) inner.chroma_site = out->height > 576 ? B200_CHROMA_SITE_H_COSITED : B200_CHROMA_SITE_NONE;
-  }
-  const bool in_422p = in->format == B200_VIDEO_FORMAT_YUY2 || in->format == B200_VIDEO_FORMAT_UYVY || in->format == B200_VIDEO_FORMAT_YVYU;
-  if (yuv && in_422p && inner.chroma_site == 0)
-    inner.chroma_site = out->height > 576 ? B200_CHROMA_SITE_H_COSITED : B200_CHROMA_SITE_NONE;
+  // colorimetry defaults belong to the whole frame, not to the rectangle: packed RGB -> 4:2:0 takes all of them, packed
+  // 4:2:2 -> 4:2:0 the chroma site
+  if (yuv && fi && fi->family == FAMILY_RGB) fill_colorimetry (&inner, *fo, out->height);
+  if (yuv && fi && fi->family == FAMILY_YUV422_PACKED && inner.chroma_site == 0)
+    inner.chroma_site = default_colorimetry (*fo, out->height).site;
   // video_converter_compute_resample (:2850-2895) compares the input with the whole output frame
   const bool forced = in->width != out->width || in->height != out->height;
   int st = build_inner_plan (in, &inner, cfg, p, forced);
@@ -858,129 +856,59 @@ int build_vcs_plan (const b200_video_info * in, const b200_video_info * out,
   p->frame_out = *out;
   p->dest[0] = dx; p->dest[1] = dy; p->dest[2] = dw; p->dest[3] = dh;
   p->fill_border = cfg->fill_border != 0;
-  return border_colour (p, *out, cfg->border_argb);
+  return border_colour (p, *fo, cfg->border_argb);
 }
 
-static int build_inner_plan (const b200_video_info * in, const b200_video_info * out,
-    const b200_vcs_config * cfg, VcsPlan * p, bool resample_forced)
+// The chain (video-converter.c:852-2112) from a YUV input: unpack, chroma up-sampling, the scalers, then the matrix to
+// packed or planar RGB, or chroma down-sampling and the 4:2:0 pack (yuv_out).
+static int build_chain_plan (VcsPlan * p, int pc, const VideoFormatDesc & fi, const VideoFormatDesc & fo,
+    bool resample_forced)
 {
-  if (!in || !out || !cfg || !p) return B200_ERR_INVALID_ARG;
-  if (in->width < 1 || in->height < 1 || out->width < 1 || out->height < 1 ||
-      in->width > 32767 || in->height > 32767 || out->width > 32767 || out->height > 32767)
-    return B200_ERR_INVALID_ARG;        // caps range [1,32767], gstvideoconvertscale.c:168-169
-  const bool in_rgb = in->format >= B200_VIDEO_FORMAT_RGBx && in->format <= B200_VIDEO_FORMAT_ABGR;
-  const bool in_422 = in->format == B200_VIDEO_FORMAT_YUY2 || in->format == B200_VIDEO_FORMAT_UYVY ||
-      in->format == B200_VIDEO_FORMAT_YVYU || in->format == B200_VIDEO_FORMAT_Y42B || in->format == B200_VIDEO_FORMAT_Y444;
-  if (in->format != B200_VIDEO_FORMAT_NV12 && in->format != B200_VIDEO_FORMAT_NV21 &&
-      in->format != B200_VIDEO_FORMAT_I420 && in->format != B200_VIDEO_FORMAT_YV12 && !in_rgb && !in_422)
-    return B200_ERR_UNSUPPORTED;
-  p->in = *in; p->out = *out; p->cfg = *cfg;
-  if (in_rgb) return build_rgb_in_plan (p);
-  if (in_422) {
+  const b200_video_info *in = &p->in, *out = &p->out;
+  p->in_422_444 = pc == PC_422_RGB || pc == PC_422_420;
+  p->yuv_out = pc == PC_420_CHAIN || pc == PC_422_420;
+  if (p->in_422_444) {
     // capture formats: unpack_YUY2 / _UYVY / _YVYU / _Y42B / _Y444 (video-format.c:155-274, :1009-1104), horizontal chroma
     // up-sampling only (4:2:2: v_factor 0 selects video_chroma_none, video-chroma.c:989-994; 4:4:4: no resampler at all),
-    // then the usual chain to packed RGB.  Generic kernel (device-verified: tests/test_vcs_rgbin_gpu.py).
-    // Packed 4:2:2 (YUY2 / UYVY / YVYU) also converts to 4:2:0 (capture -> encoder): the chain closed by chroma
-    // down-sampling, or the table rows YUY2 / UYVY -> I420 / YV12 at an unchanged size (yuy2_420 below).  Planar
-    // 4:2:2 / 4:4:4 -> planar 4:2:0 are plane-scaling table rows, -> semi-planar 4:2:0 the chain again.
-    const bool out_rgb = (out->format >= B200_VIDEO_FORMAT_RGBx && out->format <= B200_VIDEO_FORMAT_ABGR) || is_rgbp (out->format);
-    const bool out_420 =out->format == B200_VIDEO_FORMAT_I420 || out->format == B200_VIDEO_FORMAT_YV12 ||
-        out->format == B200_VIDEO_FORMAT_NV12 || out->format == B200_VIDEO_FORMAT_NV21;
-    const bool in_packed = in->format == B200_VIDEO_FORMAT_YUY2 || in->format == B200_VIDEO_FORMAT_UYVY || in->format == B200_VIDEO_FORMAT_YVYU;
-    const bool out_pl420 = out->format == B200_VIDEO_FORMAT_I420 || out->format == B200_VIDEO_FORMAT_YV12;
-    if (!in_packed && out_pl420) {
-      // planar 4:2:2 / 4:4:4 -> planar 4:2:0: plane-scaling table rows like I420 -> I420 (video-converter.c:8607-8628; the
-      // same colour matrix on both sides, :8989 - what the element's fixation produces): no chain, no chroma siting
-      if (p->in.color_matrix == 0) p->in.color_matrix = in->height > 576 ? B200_COLOR_MATRIX_BT709 : B200_COLOR_MATRIX_BT601;
-      if (p->out.color_matrix != 0 && p->out.color_matrix != p->in.color_matrix) return B200_ERR_UNSUPPORTED;
-      if (in->stride[0] < in->width || out->stride[0] < out->width) return B200_ERR_INVALID_ARG;
-      return build_planes (p, filter_from_method (*cfg));
-    }
-    // (planar 4:2:2 / 4:4:4 -> NV12 / NV21 has no table row: the chain, like the packed inputs)
-    if (!out_rgb && !out_420) return B200_ERR_UNSUPPORTED;
+    // then the usual chain.  Generic kernel (device-verified: tests/test_vcs_rgbin_gpu.py), or for 4:2:0 outputs the
+    // table rows YUY2 / UYVY -> I420 / YV12 at an unchanged size (yuy2_420 below).
     const int w = in->width;
-    p->in_422_444 = true;
     p->cvshift = 0;
-    p->chshift = in->format == B200_VIDEO_FORMAT_Y444 ? 0 : 1;
-    switch (in->format) {
-      case B200_VIDEO_FORMAT_YUY2: case B200_VIDEO_FORMAT_YVYU: case B200_VIDEO_FORMAT_UYVY: {
-        if (in->stride[0] < 4 * ((w + 1) / 2)) return B200_ERR_INVALID_ARG;
-        const int yo = in->format == B200_VIDEO_FORMAT_UYVY ? 1 : 0;
-        const int uo = in->format == B200_VIDEO_FORMAT_YUY2 ? 1 : (in->format == B200_VIDEO_FORMAT_YVYU ? 3 : 0);
-        const int vo = in->format == B200_VIDEO_FORMAT_YUY2 ? 3 : (in->format == B200_VIDEO_FORMAT_YVYU ? 1 : 2);
-        p->ystep = 2; p->cstep_in = 4;
-        p->in_off_y = in->offset[0] + yo; p->in_off_u = in->offset[0] + uo; p->in_off_v = in->offset[0] + vo;
-        p->in_stride_u = p->in_stride_v = in->stride[0];
-        break;
-      }
-      default: {
-        const int cw = p->chshift ? (w + 1) / 2 : w;
-        if (in->stride[0] < w || in->stride[1] < cw || in->stride[2] < cw) return B200_ERR_INVALID_ARG;
-        p->ystep = 1; p->cstep_in = 1;
-        p->in_off_y = in->offset[0]; p->in_off_u = in->offset[1]; p->in_off_v = in->offset[2];
-        p->in_stride_u = in->stride[1]; p->in_stride_v = in->stride[2];
-        break;
-      }
+    p->chshift = fi.wsub;
+    if (fi.family == FAMILY_YUV422_PACKED) {
+      if (in->stride[0] < 4 * ((w + 1) / 2)) return B200_ERR_INVALID_ARG;
+      p->ystep = 2; p->cstep_in = 4;
+      p->in_off_y = in->offset[0] + fi.pair_y; p->in_off_u = in->offset[0] + fi.pair_u; p->in_off_v = in->offset[0] + fi.pair_v;
+      p->in_stride_u = p->in_stride_v = in->stride[0];
+    } else {
+      const int cw = (w + fi.wsub) >> fi.wsub;
+      if (in->stride[0] < w || in->stride[fi.plane_u] < cw || in->stride[fi.plane_v] < cw) return B200_ERR_INVALID_ARG;
+      p->ystep = 1; p->cstep_in = 1;
+      p->in_off_y = in->offset[0]; p->in_off_u = in->offset[fi.plane_u]; p->in_off_v = in->offset[fi.plane_v];
+      p->in_stride_u = in->stride[fi.plane_u]; p->in_stride_v = in->stride[fi.plane_v];
     }
   }
-  // caps defaults (video-info.c:165-185, :211-225)
-  if (p->in.color_matrix == 0) p->in.color_matrix = in->height > 576 ? B200_COLOR_MATRIX_BT709 : B200_COLOR_MATRIX_BT601;
-  if (p->in.color_range == 0) p->in.color_range = B200_COLOR_RANGE_16_235;
-  if (p->in.chroma_site == 0) p->in.chroma_site = in->height > 576 ? B200_CHROMA_SITE_H_COSITED : B200_CHROMA_SITE_NONE;
-  {
-    const bool in_pl = in->format == B200_VIDEO_FORMAT_I420 || in->format == B200_VIDEO_FORMAT_YV12;
-    const bool out_pl = out->format == B200_VIDEO_FORMAT_I420 || out->format == B200_VIDEO_FORMAT_YV12;
-    const bool out_semi = out->format == B200_VIDEO_FORMAT_NV12 || out->format == B200_VIDEO_FORMAT_NV21;
-    if (out_pl || out_semi) {
-      // the reference has plane-scaling fast paths for NV12->NV12, NV21->NV21, I420/YV12 -> I420/YV12
-      // (video-converter.c:8722-8760); the other 4:2:0 pairs run the chain with chroma down-sampling
-      if (!((in_pl && out_pl) || (out_semi && in->format == out->format))) {
-        // the remaining 4:2:0 pairs have no table row: the generic chain, closed by chain_downsample
-        // (video-converter.c:2018-2032) and the 4:2:0 pack functions
-        p->yuv_out = true;
-      } else {
-        if (in->stride[0] < in->width || out->stride[0] < out->width) return B200_ERR_INVALID_ARG;
-        if (p->in.color_matrix == 0) p->in.color_matrix = in->height > 576 ? B200_COLOR_MATRIX_BT709 : B200_COLOR_MATRIX_BT601;
-        return build_planes (p, filter_from_method (*cfg));
-      }
-    }
-  }
+  fill_colorimetry (&p->in, fi, in->height);
   if (p->yuv_out) {
-    const bool out_pl = out->format == B200_VIDEO_FORMAT_I420 || out->format == B200_VIDEO_FORMAT_YV12;
-    const int ocw = (out->width + 1) / 2;
     // chain_convert (video-converter.c:1720-1868) compares the two colour matrices only (not the range): equal ->
     // no matrix stage.  A differing one would run video_orc_matrix8, whose SIMD program and C backup disagree
     // (video-orc.orc:2079-2133 vs video-converter.c:1136-1176): refused.  The element's caps fixation carries the
     // input colorimetry over to a YUV output (gstvideoconvertscale.c:1335-1427), so equal is the negotiated case.
     if (p->out.color_matrix != 0 && p->out.color_matrix != p->in.color_matrix) return B200_ERR_UNSUPPORTED;
-    // a changing sub-sampling (4:2:2 in) does not carry the input's chroma-site over (gstvideoconvertscale.c:1411-1424):
-    // the output keeps the default of its size
+    // a 4:2:0 output inherits the input's chroma site; a changing sub-sampling (4:2:2 in) does not carry it over
+    // (gstvideoconvertscale.c:1411-1424): the output keeps the default of its size
     if (p->out.chroma_site == 0)
-      p->out.chroma_site = !p->in_422_444 ? p->in.chroma_site : (out->height > 576 ? B200_CHROMA_SITE_H_COSITED : B200_CHROMA_SITE_NONE);
-    if (out->stride[0] < out->width) return B200_ERR_INVALID_ARG;
-    if (out_pl) {
-      if (out->stride[1] < ocw || out->stride[2] < ocw) return B200_ERR_INVALID_ARG;
-      p->out_plane_u = out->format == B200_VIDEO_FORMAT_YV12 ? 2 : 1;
-      p->out_plane_v = 3 - p->out_plane_u;
-      p->out_cstep = 1; p->out_u_index = 0;
-    } else {
-      if (out->stride[1] < 2 * ocw) return B200_ERR_INVALID_ARG;
-      p->out_plane_u = p->out_plane_v = 1;
-      p->out_cstep = 2; p->out_u_index = out->format == B200_VIDEO_FORMAT_NV21 ? 1 : 0;
-    }
+      p->out.chroma_site = p->in_422_444 ? default_colorimetry (fo, out->height).site : p->in.chroma_site;
+    if (!set_420_output (p, fo)) return B200_ERR_INVALID_ARG;
     { uint8_t s[4] = {0, 1, 2, 3}; memcpy (p->byte_sel, s, 4); }   // scratch pixels stay A,Y,U,V
-  } else
-  switch (out->format) {                // (A,R,G,B) component placed at each output byte
-    // RGBP / BGRP: the byte order of RGBx / BGRx puts plane k's component in byte k of the packed pixel
-    case B200_VIDEO_FORMAT_BGRA: case B200_VIDEO_FORMAT_BGRx: case B200_VIDEO_FORMAT_BGRP: { uint8_t s[4] = {3, 2, 1, 0}; memcpy (p->byte_sel, s, 4); break; }
-    case B200_VIDEO_FORMAT_RGBA: case B200_VIDEO_FORMAT_RGBx: case B200_VIDEO_FORMAT_RGBP: { uint8_t s[4] = {1, 2, 3, 0}; memcpy (p->byte_sel, s, 4); break; }
-    case B200_VIDEO_FORMAT_ABGR: case B200_VIDEO_FORMAT_xBGR: { uint8_t s[4] = {0, 3, 2, 1}; memcpy (p->byte_sel, s, 4); break; }
-    case B200_VIDEO_FORMAT_ARGB: case B200_VIDEO_FORMAT_xRGB: { uint8_t s[4] = {0, 1, 2, 3}; memcpy (p->byte_sel, s, 4); break; }
-    default: return B200_ERR_UNSUPPORTED;
+  } else {
+    // (A,R,G,B) component placed at each output byte; RGBP / BGRP: the byte order of RGBx / BGRx puts plane k's
+    // component in byte k of the packed pixel
+    for (int c = 0; c < 4; c++) p->byte_sel[fo.pos[c]] = (uint8_t) c;
   }
-  p->rgbp_out = is_rgbp (out->format);
+  p->rgbp_out = fo.family == FAMILY_RGBP;
   if (p->rgbp_out && !rgbp_strides_ok (*out)) return B200_ERR_INVALID_ARG;
-  p->planar = in->format == B200_VIDEO_FORMAT_I420 || in->format == B200_VIDEO_FORMAT_YV12;
+  p->planar = fi.family == FAMILY_YUV420;
   const int min_out_stride = (p->yuv_out || p->rgbp_out) ? out->width : out->width * 4;
   if (p->in_422_444) {
     if (out->stride[0] < min_out_stride) return B200_ERR_INVALID_ARG;
@@ -988,11 +916,10 @@ static int build_inner_plan (const b200_video_info * in, const b200_video_info *
     const int cw = (in->width + 1) / 2;
     if (in->stride[0] < in->width || in->stride[1] < cw || in->stride[2] < cw || out->stride[0] < min_out_stride)
       return B200_ERR_INVALID_ARG;
-    p->plane_u = in->format == B200_VIDEO_FORMAT_YV12 ? 2 : 1;   // YV12 keeps V in plane 1
-    p->plane_v = 3 - p->plane_u;
+    p->plane_u = fi.plane_u; p->plane_v = fi.plane_v;
   } else if (in->stride[0] < in->width || in->stride[1] < ((in->width + 1) & ~1) || out->stride[0] < min_out_stride)
     return B200_ERR_INVALID_ARG;
-  p->u_index = in->format == B200_VIDEO_FORMAT_NV21 ? 1 : 0;
+  p->u_index = fi.u_index;
   p->h_cosited = (p->in.chroma_site & B200_CHROMA_SITE_H_COSITED) != 0;
   p->v_pairs = (p->in.chroma_site & B200_CHROMA_SITE_V_COSITED) == 0 && !p->in_422_444;   // line pairs: 4:2:0 only
 
@@ -1001,7 +928,7 @@ static int build_inner_plan (const b200_video_info * in, const b200_video_info *
     if (st != B200_OK) return st;
   }
 
-  FilterSpec f = filter_from_method (*cfg);
+  FilterSpec f = filter_from_method (p->cfg);
   const int iw = in->width, ih = in->height, ow = out->width, oh = out->height;
   if (iw != ow) scaled_axis (&p->h, f, iw, ow, true); else identity_axis (&p->h, iw);
   if (ih != oh) scaled_axis (&p->v, f, ih, oh, false); else identity_axis (&p->v, ih);
@@ -1021,10 +948,10 @@ static int build_inner_plan (const b200_video_info * in, const b200_video_info *
     std::fill (p->chroma_mode.begin (), p->chroma_mode.end (), 0);
   }
   if (p->yuv_out && p->in_422_444) {
-    const bool out_pl = out->format == B200_VIDEO_FORMAT_I420 || out->format == B200_VIDEO_FORMAT_YV12;
-    // table rows YUY2 / UYVY -> I420 / YV12 (video-converter.c:8493-8507; a border rectangle disables them, :8993)
-    p->yuy2_420 = (in->format == B200_VIDEO_FORMAT_YUY2 || in->format == B200_VIDEO_FORMAT_UYVY) && out_pl &&
-        iw == ow && ih == oh && !resample_forced;
+    // table rows YUY2 / UYVY -> I420 / YV12 (video-converter.c:8493-8507, YVYU has none; a border rectangle disables
+    // them, :8993)
+    p->yuy2_420 = (in->format == B200_VIDEO_FORMAT_YUY2 || in->format == B200_VIDEO_FORMAT_UYVY) &&
+        fo.family == FAMILY_YUV420 && iw == ow && ih == oh && !resample_forced;
     if (p->yuy2_420 && out->stride[0] < 2 * ((ow + 1) / 2)) return B200_ERR_INVALID_ARG;   // whole pairs of luma per line
   }
   if (p->yuv_out) {
@@ -1074,6 +1001,35 @@ static int build_inner_plan (const b200_video_info * in, const b200_video_info *
   // directions with the 8-tap lanczos the reference derives for it
   p->lanczos2_ok = false;
   return B200_OK;
+}
+
+static int build_inner_plan (const b200_video_info * in, const b200_video_info * out,
+    const b200_vcs_config * cfg, VcsPlan * p, bool resample_forced)
+{
+  if (!in || !out || !cfg || !p) return B200_ERR_INVALID_ARG;
+  if (in->width < 1 || in->height < 1 || out->width < 1 || out->height < 1 ||
+      in->width > 32767 || in->height > 32767 || out->width > 32767 || out->height > 32767)
+    return B200_ERR_INVALID_ARG;        // caps range [1,32767], gstvideoconvertscale.c:168-169
+  const VideoFormatDesc *fi = video_format (in->format), *fo = video_format (out->format);
+  const int pc = classify (fi, fo);
+  if (pc < 0) return pc;
+  p->in = *in; p->out = *out; p->cfg = *cfg;
+  switch (pc) {
+    case PC_RGB_RGB: return build_rgb_same_plan (p, *fi, *fo);
+    case PC_RGB_RGBP: return build_rgb_rgbp_plan (p, *fi, *fo);
+    case PC_RGB_420: return build_rgb_in_plan (p, *fi, *fo);
+    case PC_PLANES:
+      if (fi->family == FAMILY_YUV_PLANAR) {
+        // planar 4:2:2 / 4:4:4 -> planar 4:2:0 name the same colour matrix on both sides (video-converter.c:8989 - what
+        // the element's fixation produces) and take no chroma siting: only the matrix default applies
+        if (p->in.color_matrix == 0) p->in.color_matrix = default_colorimetry (*fi, in->height).matrix;
+        if (p->out.color_matrix != 0 && p->out.color_matrix != p->in.color_matrix) return B200_ERR_UNSUPPORTED;
+      } else fill_colorimetry (&p->in, *fi, in->height);
+      if (in->stride[0] < in->width || out->stride[0] < out->width) return B200_ERR_INVALID_ARG;
+      return build_planes (p, *fi, *fo, filter_from_method (*cfg));
+    default:
+      return build_chain_plan (p, pc, *fi, *fo, resample_forced);
+  }
 }
 
 }  // namespace b200

@@ -61,7 +61,7 @@ def patch(text):
 def sources():
     return [os.path.join(CSRC, f) for f in ("vcs.cu", "vcs_planes.cuh", "vcs_planes_fast.cuh", "vcs_kernels.cuh", "vcs_down420.cuh", "vcs_rgb420.cuh", "vcs_yuy2_420.cuh", "vcs_l2mma.cuh", "vcs_lanczos2.cuh", "vcs_lanczos2_v2.cuh", "vcs_light.cuh",
                                             "vcs_ntap.cuh", "common.cu", "comp.cu", "ars.cu", "besi0_coeffs.inc",
-                                            "vcs_plan.cpp", "vcs_plan.h", "vcs_device.h", "common.h")] + \
+                                            "vcs_plan.cpp", "vcs_plan.h", "video_format.h", "vcs_device.h", "common.h")] + \
         [os.path.join(HERE, "emu", f) for f in sorted(os.listdir(os.path.join(HERE, "emu")))] + [os.path.abspath(__file__)]
 
 
