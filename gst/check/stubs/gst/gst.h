@@ -27,6 +27,9 @@ typedef gsize GType;
 #define CLAMP(x, lo, hi) ((x) < (lo) ? (lo) : (x) > (hi) ? (hi) : (x))
 #define G_N_ELEMENTS(a) (sizeof (a) / sizeof ((a)[0]))
 typedef struct _GList { gpointer data; struct _GList *next, *prev; } GList;
+gpointer g_malloc0 (gsize n_bytes);
+void g_free (gpointer mem);
+#define g_new0(T, n) ((T *) g_malloc0 (sizeof (T) * (n)))
 #define g_clear_pointer(pp, destroy) G_STMT_START { if (*(pp)) { (destroy) (*(pp)); *(pp) = NULL; } } G_STMT_END
 gboolean g_once_init_enter (void *location);
 void g_once_init_leave (void *location, gsize result);

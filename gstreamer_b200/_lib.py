@@ -54,6 +54,11 @@ class CompPadYuvC(C.Structure):
                 ("alpha", C.c_double), ("op", C.c_int32), ("reserved", C.c_int32)]
 
 
+class CompPadConvertC(C.Structure):
+    _fields_ = [("data", C.c_void_p), ("info", VideoInfoC), ("conv", C.c_void_p), ("xpos", C.c_int32), ("ypos", C.c_int32),
+                ("alpha", C.c_double), ("op", C.c_int32), ("reserved", C.c_int32)]
+
+
 class ArsConfigC(C.Structure):
     _fields_ = [("in_rate", C.c_int32), ("out_rate", C.c_int32), ("channels", C.c_int32),
                 ("quality", C.c_int32), ("format", C.c_int32), ("resample_method", C.c_int32),
@@ -107,6 +112,7 @@ _SIGS = {
     "b200_comp_blend_yuv_host": (C.c_int, [_P, _P, C.POINTER(VideoInfoC), C.c_int, C.POINTER(CompPadYuvC), C.c_int]),
     "b200_comp_blend_host": (C.c_int, [_P, _P, C.c_int32, C.c_int, C.POINTER(CompPadC), C.c_int]),
     "b200_comp_blend_yuv": (C.c_int, [_P, _P, C.POINTER(VideoInfoC), C.c_int, C.POINTER(CompPadYuvC), C.c_int, _P]),
+    "b200_comp_blend_convert": (C.c_int, [_P, _P, C.POINTER(VideoInfoC), C.c_int, C.POINTER(CompPadConvertC), C.c_int, _P]),
     "b200_ars_create": (C.c_int, [C.POINTER(ArsConfigC), C.c_int, C.POINTER(_P)]),
     "b200_ars_destroy": (None, [_P]),
     "b200_ars_reset": (C.c_int, [_P]),

@@ -62,11 +62,11 @@ def pad_output_size(src_w, src_h, pad_w, pad_h, sizing_policy="none", zero_size_
 
 class CudaCompositorPad:
     """GstCompositorPad.  `width`/`height` are the pad properties (compositor.c:190-196): the size the
-    pad's picture takes in the output.  With `in_info` the pad is a GstVideoAggregatorConvertPad: its
-    input frames (NV12/NV21/I420/YV12 of any size) are converted to the aggregator's format and scaled to
-    width x height in prepare_frame (gstvideoaggregator.c:479-570, :782-830) by a GstVideoConverter with
-    DEFAULT options — cubic b = c = 1/3 (video-converter.c:791, video-resampler.c:63-64), i.e. exactly
-    cudavideoconvertscale method=mitchell — before blending."""
+    pad's picture takes in the output.  `in_info` is the pad's caps: the pad is a GstVideoAggregatorConvertPad and its
+    frames are converted to the aggregator's format, colorimetry and chroma site at width x height
+    (gstvideoaggregator.c:479-570, :782-830) by a GstVideoConverter with DEFAULT options - cubic b = c = 1/3
+    (video-converter.c:791, video-resampler.c:63-64), i.e. exactly cudavideoconvertscale method=mitchell - when that
+    conversion differs from the caps.  The conversion runs inside b200_comp_blend_convert."""
 
     def __init__(self, width, height, stride=None, xpos=0, ypos=0, alpha=1.0, operator=Operator.OVER, in_info=None,
                  sizing_policy="none"):
@@ -80,28 +80,25 @@ class CudaCompositorPad:
         self.width, self.height = width, height
         self.stride = stride or width * 4
         self.xpos, self.ypos, self.alpha, self.operator = xpos, ypos, alpha, Operator(operator)
-        self.frame = None          # the pad's prepared frame (device memory)
+        self.frame = None          # the pad's frame (device memory)
         self.in_info = in_info
-        self._conv = self._converted = None
 
     def set_frame(self, frame):
         self.frame = frame
         return self
 
-    def _prepare_frame(self, out_format, device, stream):
-        """prepare_frame of a convert pad: returns the frame to blend"""
-        if self.in_info is None or self.frame is None:
-            return self.frame
-        import torch
-        from .video import CudaVideoConvertScale, VideoInfo, VideoScaleMethod
-        if self._conv is None:
-            self._conv = CudaVideoConvertScale(add_borders=False, method=VideoScaleMethod.MITCHELL, cuda_device_id=device)
-            self._out_info = VideoInfo(out_format, self.width, self.height)
-            self._conv.set_info(self.in_info, self._out_info)
-            self._converted = torch.empty(self._out_info.size, dtype=torch.uint8, device=f"cuda:{device}")
-            self.stride = self._out_info.stride[0]
-        self._conv.transform_frame(self.frame, self._converted, stream)
-        return self._converted
+    def conversion_info(self, out_info):
+        """gst_video_aggregator_convert_pad_create_conversion_info + gst_compositor_pad_create_conversion_info: the
+        aggregator's format, colorimetry and chroma site at the pad's output size; None when that is the pad's caps"""
+        from .video import VideoInfo
+        if self.in_info is None:
+            return None
+        conv = VideoInfo(out_info.format, self.width, self.height)
+        conv.set_colorimetry(out_info.c.color_matrix, out_info.c.color_range, out_info.c.chroma_site)
+        a, b = self.in_info.c, conv.c
+        same = (a.format, a.width, a.height, a.color_matrix, a.color_range, a.chroma_site) == \
+            (b.format, b.width, b.height, b.color_matrix, b.color_range, b.chroma_site)
+        return None if same else conv
 
 
 class CudaCompositor:
@@ -110,6 +107,7 @@ class CudaCompositor:
         self.width, self.height, self.format = width, height, VideoFormat(out_format)
         self.sinkpads = []
         self.device = cuda_device_id
+        self._convs = {}           # one converter per distinct (pad caps, conversion info): pads that share it batch
         h = C.c_void_p()
         check(lib.b200_comp_create(int(out_format), width, height, cuda_device_id, C.byref(h)),
               "b200_comp_create")
@@ -124,35 +122,48 @@ class CudaCompositor:
                    VideoFormat.I420_10LE, VideoFormat.I420_12LE, VideoFormat.I422_10LE, VideoFormat.I422_12LE,
                    VideoFormat.Y444_10LE, VideoFormat.Y444_12LE, VideoFormat.Y444_16LE)
 
-    def _aggregate_yuv(self, outbuf, out_info, stream):
-        """4:2:0 output: every pad frame has the output's format (blend.c PLANAR_YUV_BLEND / NV_YUV_BLEND);
-        a pad's plane layout comes from pad.in_info, default layout otherwise"""
+    @staticmethod
+    def _key(info):
+        c = info.c
+        return (c.format, c.width, c.height, tuple(c.stride), tuple(c.offset), c.color_matrix, c.color_range, c.chroma_site)
+
+    def _converter(self, in_info, conv_info, used):
+        from .video import CudaVideoConvertScale, VideoScaleMethod
+        key = (self._key(in_info), self._key(conv_info))
+        if key not in self._convs:
+            conv = CudaVideoConvertScale(add_borders=False, method=VideoScaleMethod.MITCHELL, cuda_device_id=self.device)
+            conv.set_info(in_info, conv_info)
+            self._convs[key] = conv
+        used[key] = self._convs[key]
+        return self._convs[key]
+
+    # GstVideoAggregatorClass::aggregate_frames (outbuf is device memory).  out_info: the output's plane layout and
+    # colorimetry (default layout otherwise); out_stride: the row stride of a packed RGB output.
+    def aggregate_frames(self, outbuf, out_stride=None, stream=None, out_info=None):
         from .video import VideoInfo
-        out_info = out_info or VideoInfo(self.format, self.width, self.height)
+        if out_info is None:
+            out_info = VideoInfo(self.format, self.width, self.height)
+            if self.format not in self.YUV_FORMATS and out_stride:
+                out_info.set_layout([out_stride], [0])
         pads = [p for p in self.sinkpads if p.frame is not None]
-        arr = (_lib.CompPadYuvC * max(len(pads), 1))()
-        keep = []
+        arr = (_lib.CompPadConvertC * max(len(pads), 1))()
+        used = {}
         for i, p in enumerate(pads):
-            info = p.in_info or VideoInfo(self.format, p.width, p.height)
-            keep.append(info)
+            conv_info = p.conversion_info(out_info)
+            if p.in_info is not None:
+                info = p.in_info
+            else:
+                info = VideoInfo(self.format, p.width, p.height)
+                if self.format not in self.YUV_FORMATS:
+                    info.set_layout([p.stride], [0])
             arr[i].data = _ptr(p.frame)
             arr[i].info = info.c
+            arr[i].conv = self._converter(info, conv_info, used)._h if conv_info is not None else None
             arr[i].xpos, arr[i].ypos, arr[i].alpha, arr[i].op = p.xpos + p.x_offset, p.ypos + p.y_offset, p.alpha, int(p.operator)
-        check(lib.b200_comp_blend_yuv(self._h, _ptr(outbuf), C.byref(out_info.c), int(self.background), arr, len(pads),
-                                      _stream(stream)), "b200_comp_blend_yuv")
-
-    # GstVideoAggregatorClass::aggregate_frames (outbuf is device memory)
-    def aggregate_frames(self, outbuf, out_stride=None, stream=None, out_info=None):
-        if self.format in self.YUV_FORMATS:
-            return self._aggregate_yuv(outbuf, out_info, stream)
-        pads = [p for p in self.sinkpads if p.frame is not None]
-        arr = (_lib.CompPadC * max(len(pads), 1))()
-        for i, p in enumerate(pads):
-            arr[i].data = _ptr(p._prepare_frame(self.format, self.device, stream))
-            arr[i].width, arr[i].height, arr[i].stride = p.width, p.height, p.stride
-            arr[i].xpos, arr[i].ypos, arr[i].alpha, arr[i].op = p.xpos + p.x_offset, p.ypos + p.y_offset, p.alpha, int(p.operator)
-        check(lib.b200_comp_blend(self._h, _ptr(outbuf), out_stride or self.width * 4, int(self.background),
-                                  arr, len(pads), _stream(stream)), "b200_comp_blend")
+        check(lib.b200_comp_blend_convert(self._h, _ptr(outbuf), C.byref(out_info.c), int(self.background), arr, len(pads),
+                                          _stream(stream)), "b200_comp_blend_convert")
+        # a converter no pad uses any more (a pad's caps or size changed) is destroyed (its cudaFree waits for the call)
+        self._convs = used
 
     # system-memory peers: pad frames and the output are HOST buffers (addresses); see b200_comp_blend_host_submit
     def aggregate_host_frames(self, out_ptr, pad_ptrs, out_stride=None, wait=True):

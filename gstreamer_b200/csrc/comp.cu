@@ -12,6 +12,7 @@
 // (the reference moves bg write + per pad src read + dst read + dst write).
 #include "common.h"
 #include "video_format.h"
+#include "vcs_device.h"
 
 #include <string.h>
 #include <algorithm>
@@ -351,7 +352,138 @@ struct b200_comp {
   CompHostSlot slot[kSlots];
   cudaStream_t s_h2d = nullptr, s_run = nullptr, s_d2h = nullptr;
   unsigned long long submitted = 0;
+  uint8_t *d_conv = nullptr;     // b200_comp_blend_convert: the two-pass pads' converted frames
+  size_t conv_cap = 0;
 };
+
+// The 4:2:0 compositor's launches (b200_comp_blend_yuv, b200_comp_blend_convert): pads are collected in z-order and flushed
+// in chunks of CY_MAX_PADS; the first launch draws the background, later ones continue from the destination.
+struct YuvBlend {
+  b200_comp *h = nullptr;
+  CompYuvParams P;
+  dim3 grid;
+  cudaStream_t stream = nullptr;
+  int launched = 0;
+  int W = 0, H = 0, ws = 0, hs = 0, xr = 1, yr = 1, es = 1, nbits = 8, n_planes = 0;
+  bool semi = false;
+
+  static int sub (int v, int sh) { return -((-v) >> sh); }        // GST_VIDEO_FORMAT_INFO_SCALE_WIDTH / _HEIGHT (round up)
+
+  int init (b200_comp * hh, void *dst, const b200_video_info * di, int background, cudaStream_t s)
+  {
+    h = hh; stream = s;
+    // the format's PLANAR_YUV_BLEND / NV_YUV_BLEND instantiation (blend.c:591-646, :1386): chroma sub-sampling shifts,
+    // bytes per sample and depth from the format table; the position rounds up to the chroma grid (x_round / y_round)
+    const b200::VideoFormatDesc & d = *b200::video_format (h->format);
+    semi = d.family == b200::FAMILY_NV;
+    ws = d.wsub; hs = d.hsub; xr = 1 << ws; yr = 1 << hs; es = d.bytes; nbits = d.depth;
+    W = h->width; H = h->height; n_planes = d.n_planes;
+    memset (&P, 0, sizeof (P));
+    P.n_planes = n_planes; P.es = es; P.nbits = nbits;
+    for (int p = 0; p < n_planes; p++) {
+      P.dst[p] = (uint8_t *) dst + di->offset[p];
+      P.stride[p] = di->stride[p];
+      P.wbytes[p] = (p == 0 ? W : (semi ? 2 * sub (W, ws) : sub (W, ws))) * es;
+      P.rows[p] = p == 0 ? H : sub (H, hs);
+      if (P.stride[p] < P.wbytes[p]) return B200_ERR_INVALID_ARG;
+      if (es == 2 && ((P.stride[p] & 1) || (di->offset[p] & 1))) return B200_ERR_INVALID_ARG;
+      // _draw_background (compositor.c:1619-1675): checker = luma squares + mid-grey chroma; black / white from the range
+      // offsets at the format's depth (compositor.c:1131-1149, gst_video_color_range_offsets video-color.c:204-252: 16-235 ->
+      // 16 << (n - 8) .. 235 << (n - 8); 0-255 -> 0 .. 2^n - 1; chroma 1 << (n - 1)); transparent = zeroed planes
+      const bool full_range = di->color_range == B200_COLOR_RANGE_0_255;
+      const int mid = 1 << (nbits - 1);
+      if (background == B200_COMP_BG_CHECKER) { P.bg_mode[p] = p == 0 ? 0 : 1; P.bg_value[p] = mid; }
+      else if (background == B200_COMP_BG_TRANSPARENT) { P.bg_mode[p] = 1; P.bg_value[p] = 0; }
+      else {
+        P.bg_mode[p] = 1;
+        P.bg_value[p] = p ? mid : (background == B200_COMP_BG_BLACK ? (full_range ? 0 : 16 << (nbits - 8))
+                                                                    : (full_range ? (1 << nbits) - 1 : 235 << (nbits - 8)));
+      }
+    }
+    unsigned gx = 0, gy = 0;
+    for (int p = 0; p < n_planes; p++) {
+      gx = std::max (gx, (unsigned) ((P.wbytes[p] + 127) / 128));
+      gy = std::max (gy, (unsigned) ((P.rows[p] + 7) / 8));
+    }
+    grid = dim3 (gx, gy, n_planes);
+    return B200_OK;
+  }
+
+  int flush ()
+  {
+    comp_yuv_kernel <<<grid, 256, 0, stream>>> (P);
+    B200_CUDA_TRY (cudaGetLastError ());
+    launched++;
+    P.n_pads = 0;
+    for (int p = 0; p < n_planes; p++) P.bg_mode[p] = -1;           // later chunks continue from the destination
+    return B200_OK;
+  }
+
+  // the blend's alpha of a pad: 0 = skipped, CY_COPY = copied (alpha 1.0, or SOURCE: _blend_* copies in source mode)
+  int pad_alpha (double alpha, int op) const
+  {
+    if (op == B200_COMP_OP_SOURCE) alpha = 1.0;
+    if (alpha == 0.0) return 0;
+    if (alpha == 1.0) return CY_COPY;
+    const int range = (1 << nbits) - 1;
+    const int a = (int) (alpha * range);
+    return a < 0 ? 0 : (a > range ? range : a);
+  }
+
+  // blend_<format> (blend.c:284-340 / :1418-1470): the position rounded UP to the format's grid; false when the pad lies
+  // outside the frame.  x0 .. y1: the luma rectangle it covers.
+  bool place (int xpos_in, int ypos_in, int w, int hgt, int *xpos, int *ypos, int *x0, int *y0, int *x1, int *y1) const
+  {
+    *xpos = (xpos_in + xr - 1) & ~(xr - 1); *ypos = (ypos_in + yr - 1) & ~(yr - 1);
+    *x0 = std::max (*xpos, 0); *y0 = std::max (*ypos, 0);
+    *x1 = std::min (*xpos + w, W); *y1 = std::min (*ypos + hgt, H);
+    return *x1 > *x0 && *y1 > *y0;
+  }
+
+  int add (const void *data, const b200_video_info & info, int xpos_in, int ypos_in, double alpha, int op)
+  {
+    const int b_alpha = pad_alpha (alpha, op);
+    if (b_alpha == 0) return B200_OK;
+    int xpos, ypos, x0, y0, x1, y1;
+    if (!place (xpos_in, ypos_in, info.width, info.height, &xpos, &ypos, &x0, &y0, &x1, &y1)) return B200_OK;
+    const int xoffset = x0 - xpos, yoffset = y0 - ypos, bw = x1 - x0, bh = y1 - y0;
+    xpos = x0; ypos = y0;
+    if (P.n_pads == CY_MAX_PADS) { int st = flush (); if (st != B200_OK) return st; }
+    // chroma: widths and x positions by SCALE_WIDTH (round up), rows by a plain shift (blend.c:371-376)
+    const int cw = sub (bw, ws), ch = sub (bh, hs);
+    const int cxpos = xpos ? sub (xpos, ws) : 0, cypos = ypos >> hs, cxoff = xoffset ? sub (xoffset, ws) : 0, cyoff = yoffset >> hs;
+    for (int p = 0; p < n_planes; p++) {
+      CompYuvRect & r = P.pads[P.n_pads][p];
+      const int mul = ((p && semi) ? 2 : 1) * es;                   // plane bytes per (chroma) sample position
+      const int px = p ? mul * cxpos : es * xpos, py = p ? cypos : ypos, sx = p ? mul * cxoff : es * xoffset, sy = p ? cyoff : yoffset;
+      const int w = p ? mul * cw : es * bw, hgt = p ? ch : bh;
+      r.stride = info.stride[p];
+      if (es == 2 && ((r.stride & 1) || (info.offset[p] & 1) || (((uintptr_t) data) & 1))) return B200_ERR_INVALID_ARG;
+      r.x0 = px; r.x1 = px + w; r.y0 = py; r.y1 = py + hgt; r.alpha = b_alpha;
+      r.src = (const uint8_t *) data + info.offset[p] + (long long) (sy - py) * r.stride + (sx - px);
+    }
+    P.n_pads++;
+    return B200_OK;
+  }
+
+  // the pads collected so far; the background alone when nothing was launched yet
+  int finish () { return P.n_pads > 0 || launched == 0 ? flush () : B200_OK; }
+};
+
+
+// How b200_comp_blend_convert treats a pad
+enum PadRoute { PR_SKIP, PR_BLEND, PR_FUSED, PR_TWO_PASS };
+
+// The one place that decides it, from the pad's converter (none, or whether its plan scales planes into the output's
+// 8-bit 4:2:0 format: vcs_comp_fusable), the output family, the alpha the blend would use (0: dropped, before any
+// conversion, compositor.c:547-550) and whether the pad's clipped rectangle is empty
+PadRoute pad_route (const b200_vcs * conv, bool yuv420_out, int blend_alpha, bool visible)
+{
+  if (blend_alpha == 0 || !visible) return PR_SKIP;
+  if (!conv) return PR_BLEND;                                      // comp_kernel / comp_yuv_kernel, as b200_comp_blend[_yuv]
+  if (yuv420_out && b200::vcs_comp_fusable (conv)) return PR_FUSED;   // the plane scalers store into the destination
+  return PR_TWO_PASS;                                              // b200_vcs_convert_batch into d_conv, then the blend kernel
+}
 
 extern "C" {
 
@@ -393,6 +525,10 @@ void b200_comp_destroy (b200_comp * h)
       if (sl.ev_out) cudaEventDestroy (sl.ev_out);
     }
     cudaStreamDestroy (h->s_h2d); cudaStreamDestroy (h->s_run); cudaStreamDestroy (h->s_d2h);
+  }
+  if (h->device >= 0 && h->d_conv) {
+    DeviceGuard g (h->device);
+    cudaFree (h->d_conv);
   }
   delete h;
 }
@@ -460,89 +596,152 @@ int b200_comp_blend_yuv (b200_comp * h, void *dst, const b200_video_info * di, i
   if (h->device < 0) return B200_ERR_NO_DEVICE;
   DeviceGuard g (h->device);
   if (!g.ok) return B200_ERR_CUDA;
-  // the format's PLANAR_YUV_BLEND / NV_YUV_BLEND instantiation (blend.c:591-646, :1386): chroma sub-sampling shifts,
-  // bytes per sample and depth from the format table; the position rounds up to the chroma grid (x_round / y_round)
-  const b200::VideoFormatDesc & d = *b200::video_format (h->format);
-  const bool semi = d.family == b200::FAMILY_NV;
-  const int ws = d.wsub, hs = d.hsub, xr = 1 << ws, yr = 1 << hs, es = d.bytes, nbits = d.depth;
-  const int W = h->width, H = h->height, n_planes = d.n_planes;
-  auto sub = [] (int v, int sh) { return -((-v) >> sh); };         // GST_VIDEO_FORMAT_INFO_SCALE_WIDTH / _HEIGHT (round up)
-  CompYuvParams P;
-  memset (&P, 0, sizeof (P));
-  P.n_planes = n_planes; P.es = es; P.nbits = nbits;
-  for (int p = 0; p < n_planes; p++) {
-    P.dst[p] = (uint8_t *) dst + di->offset[p];
-    P.stride[p] = di->stride[p];
-    P.wbytes[p] = (p == 0 ? W : (semi ? 2 * sub (W, ws) : sub (W, ws))) * es;
-    P.rows[p] = p == 0 ? H : sub (H, hs);
-    if (P.stride[p] < P.wbytes[p]) return B200_ERR_INVALID_ARG;
-    if (es == 2 && ((P.stride[p] & 1) || (di->offset[p] & 1))) return B200_ERR_INVALID_ARG;
-    // _draw_background (compositor.c:1619-1675): checker = luma squares + mid-grey chroma; black / white from the range
-    // offsets at the format's depth (compositor.c:1131-1149, gst_video_color_range_offsets video-color.c:204-252: 16-235 ->
-    // 16 << (n - 8) .. 235 << (n - 8); 0-255 -> 0 .. 2^n - 1; chroma 1 << (n - 1)); transparent = zeroed planes
-    const bool full_range = di->color_range == B200_COLOR_RANGE_0_255;
-    const int mid = 1 << (nbits - 1);
-    if (background == B200_COMP_BG_CHECKER) { P.bg_mode[p] = p == 0 ? 0 : 1; P.bg_value[p] = mid; }
-    else if (background == B200_COMP_BG_TRANSPARENT) { P.bg_mode[p] = 1; P.bg_value[p] = 0; }
-    else {
-      P.bg_mode[p] = 1;
-      P.bg_value[p] = p ? mid : (background == B200_COMP_BG_BLACK ? (full_range ? 0 : 16 << (nbits - 8))
-                                                                  : (full_range ? (1 << nbits) - 1 : 235 << (nbits - 8)));
-    }
-  }
-  unsigned gx = 0, gy = 0;
-  for (int p = 0; p < n_planes; p++) {
-    gx = std::max (gx, (unsigned) ((P.wbytes[p] + 127) / 128));
-    gy = std::max (gy, (unsigned) ((P.rows[p] + 7) / 8));
-  }
-  const dim3 grid (gx, gy, n_planes);
-  int launched = 0;
-  auto flush = [&] () -> int {
-    comp_yuv_kernel <<<grid, 256, 0, (cudaStream_t) cuda_stream>>> (P);
-    B200_CUDA_TRY (cudaGetLastError ());
-    launched++;
-    P.n_pads = 0;
-    for (int p = 0; p < n_planes; p++) P.bg_mode[p] = -1;           // later chunks continue from the destination
-    return B200_OK;
-  };
-  const int range = (1 << nbits) - 1;
+  YuvBlend B;
+  int st = B.init (h, dst, di, background, (cudaStream_t) cuda_stream);
+  if (st != B200_OK) return st;
   for (int i = 0; i < n_pads; i++) {
     const b200_comp_pad_yuv & pad = pads[i];
     if (pad.info.format != h->format || pad.info.width < 1 || pad.info.height < 1 || !pad.data) return B200_ERR_INVALID_ARG;
-    double alpha = pad.alpha;
-    if (pad.op == B200_COMP_OP_SOURCE) alpha = 1.0;                // _blend_*: source mode copies
-    if (alpha == 0.0) continue;
-    // blend_<format> (blend.c:284-340 / :1418-1470): position rounded UP to the format's grid, clip against the frame
-    int xpos = (pad.xpos + xr - 1) & ~(xr - 1), ypos = (pad.ypos + yr - 1) & ~(yr - 1), xoffset = 0, yoffset = 0;
-    int bw = pad.info.width, bh = pad.info.height;
-    if (xpos < 0) { xoffset = -xpos; bw -= -xpos; xpos = 0; }
-    if (ypos < 0) { yoffset = -ypos; bh -= -ypos; ypos = 0; }
-    if (xoffset >= pad.info.width || yoffset >= pad.info.height) continue;
-    if (xpos + bw > W) bw = W - xpos;
-    if (ypos + bh > H) bh = H - ypos;
-    if (bw <= 0 || bh <= 0) continue;
-    int b_alpha = CY_COPY;
-    if (alpha != 1.0) { b_alpha = (int) (alpha * range); b_alpha = b_alpha < 0 ? 0 : (b_alpha > range ? range : b_alpha); }
-    if (P.n_pads == CY_MAX_PADS) { int st = flush (); if (st != B200_OK) return st; }
-    // chroma: widths and x positions by SCALE_WIDTH (round up), rows by a plain shift (blend.c:371-376)
-    const int cw = sub (bw, ws), ch = sub (bh, hs);
-    const int cxpos = xpos ? sub (xpos, ws) : 0, cypos = ypos >> hs, cxoff = xoffset ? sub (xoffset, ws) : 0, cyoff = yoffset >> hs;
-    for (int p = 0; p < n_planes; p++) {
-      CompYuvRect & r = P.pads[P.n_pads][p];
-      const int mul = ((p && semi) ? 2 : 1) * es;                   // plane bytes per (chroma) sample position
-      const int px = p ? mul * cxpos : es * xpos, py = p ? cypos : ypos, sx = p ? mul * cxoff : es * xoffset, sy = p ? cyoff : yoffset;
-      const int w = p ? mul * cw : es * bw, hgt = p ? ch : bh;
-      r.stride = pad.info.stride[p];
-      if (es == 2 && ((r.stride & 1) || (pad.info.offset[p] & 1) || (((uintptr_t) pad.data) & 1))) return B200_ERR_INVALID_ARG;
-      r.x0 = px; r.x1 = px + w; r.y0 = py; r.y1 = py + hgt; r.alpha = b_alpha;
-      r.src = (const uint8_t *) pad.data + pad.info.offset[p] + (long long) (sy - py) * r.stride + (sx - px);
-    }
-    P.n_pads++;
+    if ((st = B.add (pad.data, pad.info, pad.xpos, pad.ypos, pad.alpha, pad.op)) != B200_OK) return st;
   }
-  if (P.n_pads > 0 || launched == 0) { int st = flush (); if (st != B200_OK) return st; }
-  return B200_OK;
+  return B.finish ();
 }
+int b200_comp_blend_convert (b200_comp * h, void *dst, const b200_video_info * di, int background,
+    const b200_comp_pad_convert * pads, int n_pads, void *cuda_stream)
+{
+  if (!h || !dst || !di || n_pads < 0 || n_pads > B200_COMP_MAX_PADS || (n_pads && !pads)) return B200_ERR_INVALID_ARG;
+  if (background < 0 || background > 3) return B200_ERR_INVALID_ARG;
+  if (di->format != h->format || di->width != h->width || di->height != h->height) return B200_ERR_INVALID_ARG;
+  if (h->device < 0) return B200_ERR_NO_DEVICE;
+  DeviceGuard g (h->device);
+  if (!g.ok) return B200_ERR_CUDA;
+  const cudaStream_t stream = (cudaStream_t) cuda_stream;
+  const bool rgb = h->alpha_shift >= 0;
+  const b200::VideoFormatDesc & fd = *b200::video_format (h->format);
+  const bool yuv420 = !rgb && (fd.family == b200::FAMILY_YUV420 || fd.family == b200::FAMILY_NV) && fd.bytes == 1;
+  int st;
+  YuvBlend B;
+  if (!rgb && (st = B.init (h, dst, di, background, stream)) != B200_OK) return st;
 
+  // every pad's route; the two-pass pads' converted frames one after another in d_conv (256-byte aligned)
+  PadRoute route[B200_COMP_MAX_PADS];
+  int xr[B200_COMP_MAX_PADS], yr[B200_COMP_MAX_PADS], rect[B200_COMP_MAX_PADS][4], alpha[B200_COMP_MAX_PADS];
+  size_t off[B200_COMP_MAX_PADS], need = 0;
+  for (int i = 0; i < n_pads; i++) {
+    const b200_comp_pad_convert & pad = pads[i];
+    const b200_video_info & in = pad.info;
+    if (!pad.data || in.width < 1 || in.height < 1) return B200_ERR_INVALID_ARG;
+    if (pad.conv) {
+      const b200_video_info & ci = b200::vcs_in_info (pad.conv);
+      if (b200::vcs_device (pad.conv) != h->device || b200::vcs_out_info (pad.conv).format != h->format || ci.format != in.format || ci.width != in.width ||
+          ci.height != in.height || memcmp (ci.stride, in.stride, sizeof (in.stride)) || memcmp (ci.offset, in.offset, sizeof (in.offset)))
+        return B200_ERR_INVALID_ARG;
+    } else if (in.format != h->format) {
+      return B200_ERR_INVALID_ARG;
+    }
+    const b200_video_info & fi = pad.conv ? b200::vcs_out_info (pad.conv) : in;     // the frame the blend sees
+    bool visible;
+    if (rgb) {
+      // s_alpha = CLAMP ((gint) (alpha * 255), 0, 255), as b200_comp_blend
+      const int a = (int) (pad.alpha * 255);
+      alpha[i] = a < 0 ? 0 : (a > 255 ? 255 : a);
+      visible = pad.xpos < h->width && pad.ypos < h->height && pad.xpos + fi.width > 0 && pad.ypos + fi.height > 0;
+    } else {
+      alpha[i] = B.pad_alpha (pad.alpha, pad.op);
+      visible = B.place (pad.xpos, pad.ypos, fi.width, fi.height, &xr[i], &yr[i], &rect[i][0], &rect[i][1], &rect[i][2], &rect[i][3]);
+    }
+    route[i] = pad_route (pad.conv, yuv420, alpha[i], visible);
+    if (route[i] == PR_TWO_PASS) {
+      off[i] = need;
+      need += (b200_video_info_size (&fi) + 255) & ~(size_t) 255;
+    }
+  }
+  if (need > h->conv_cap) {
+    B200_CUDA_TRY (cudaFree (h->d_conv));                           // synchronises with blends still reading it
+    h->d_conv = nullptr; h->conv_cap = 0;
+    B200_CUDA_TRY (cudaMalloc ((void **) &h->d_conv, need));
+    h->conv_cap = need;
+  }
+  // two-pass pads: one batch per converter
+  bool done[B200_COMP_MAX_PADS] = {false};
+  for (int i = 0; i < n_pads; i++) {
+    if (route[i] != PR_TWO_PASS || done[i]) continue;
+    const void *in[B200_COMP_MAX_PADS];
+    void *out[B200_COMP_MAX_PADS];
+    int n = 0;
+    for (int j = i; j < n_pads; j++)
+      if (route[j] == PR_TWO_PASS && pads[j].conv == pads[i].conv) {
+        in[n] = pads[j].data; out[n] = h->d_conv + off[j]; n++;
+        done[j] = true;
+      }
+    if ((st = b200_vcs_convert_batch (pads[i].conv, n, in, out, cuda_stream)) != B200_OK) return st;
+  }
+  auto blend_data = [&] (int i) -> const uint8_t * {
+    return route[i] == PR_TWO_PASS ? h->d_conv + off[i] : (const uint8_t *) pads[i].data;
+  };
+  auto blend_info = [&] (int i) -> const b200_video_info & {
+    return pads[i].conv ? b200::vcs_out_info (pads[i].conv) : pads[i].info;
+  };
+
+  if (rgb) {
+    b200_comp_pad cp[B200_COMP_MAX_PADS];
+    int n = 0;
+    for (int i = 0; i < n_pads; i++) {
+      if (route[i] == PR_SKIP) continue;
+      const b200_video_info & fi = blend_info (i);
+      b200_comp_pad & c = cp[n++];
+      c.data = blend_data (i) + fi.offset[0];
+      c.width = fi.width; c.height = fi.height; c.stride = fi.stride[0];
+      c.xpos = pads[i].xpos; c.ypos = pads[i].ypos; c.alpha = pads[i].alpha; c.op = pads[i].op; c.reserved = 0;
+    }
+    return b200_comp_blend (h, (uint8_t *) dst + di->offset[0], di->stride[0], background, cp, n, cuda_stream);
+  }
+
+  // 4:2:0 and the other planar outputs: z-order runs.  A run of blend-kernel pads is one comp_yuv_kernel launch (per
+  // CY_MAX_PADS), a run of fused pads one plane-scaler launch per group: pads of one converter that overlap no pad of
+  // their own group or of a group launched after it
+  int groups = 0, gconv_first[B200_COMP_MAX_PADS], gn[B200_COMP_MAX_PADS], gpad[B200_COMP_MAX_PADS][B200_COMP_MAX_PADS];
+  auto overlap = [&] (int a, int b) {
+    return rect[a][0] < rect[b][2] && rect[b][0] < rect[a][2] && rect[a][1] < rect[b][3] && rect[b][1] < rect[a][3];
+  };
+  auto flush_fused = [&] () -> int {
+    for (int k = 0; k < groups; k++) {
+      CompStore S;
+      const uint8_t *in[B200_VCS_MAX_BATCH];
+      for (int p = 0; p < 3; p++) { S.dw[p] = B.P.wbytes[p]; S.dh[p] = B.P.rows[p]; }
+      for (int j = 0; j < gn[k]; j++) {
+        const int i = gpad[k][j];
+        in[j] = (const uint8_t *) pads[i].data;
+        S.alpha[j] = alpha[i] == CY_COPY ? 256 : alpha[i];
+        S.px[0][j] = xr[i]; S.py[0][j] = yr[i];
+        for (int p = 1; p < 3; p++) { S.px[p][j] = (xr[i] >> 1) * (B.semi ? 2 : 1); S.py[p][j] = yr[i] >> 1; }
+      }
+      const int s = b200::vcs_comp_launch (pads[gconv_first[k]].conv, gn[k], in, (uint8_t *) dst, *di, S, stream);
+      if (s != B200_OK) return s;
+    }
+    groups = 0;
+    return B200_OK;
+  };
+  for (int i = 0; i < n_pads; i++) {
+    if (route[i] == PR_SKIP) continue;
+    if (route[i] != PR_FUSED) {
+      if ((st = flush_fused ()) != B200_OK) return st;
+      if ((st = B.add (blend_data (i), blend_info (i), pads[i].xpos, pads[i].ypos, pads[i].alpha, pads[i].op)) != B200_OK) return st;
+      continue;
+    }
+    if (B.P.n_pads > 0 || B.launched == 0)                         // what lies below: the background, the blend run
+      if ((st = B.finish ()) != B200_OK) return st;
+    int g = groups - 1;
+    while (g >= 0 && pads[gconv_first[g]].conv != pads[i].conv) g--;
+    for (int k = g; g >= 0 && k < groups; k++)
+      for (int j = 0; j < gn[k]; j++)
+        if (overlap (i, gpad[k][j])) { g = -1; break; }
+    if (g < 0) { g = groups++; gconv_first[g] = i; gn[g] = 0; }
+    gpad[g][gn[g]++] = i;
+  }
+  if ((st = flush_fused ()) != B200_OK) return st;
+  return B.finish ();
+}
 
 static int comp_host_ready (b200_comp * h)
 {

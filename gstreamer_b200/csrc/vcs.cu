@@ -559,6 +559,35 @@ int ensure_pipeline (b200_vcs * h, int chunk)
 
 }  // namespace
 
+namespace b200 {
+
+bool vcs_comp_fusable (const b200_vcs * h)
+{
+  const VcsPlan & p = h->plan;
+  const VideoFormatDesc & d = *video_format (p.out.format);
+  return h->device >= 0 && p.planes_mode && !p.has_dest && (d.family == FAMILY_YUV420 || d.family == FAMILY_NV) && d.bytes == 1;
+}
+
+int vcs_device (const b200_vcs * h) { return h->device; }
+const b200_video_info & vcs_in_info (const b200_vcs * h) { return h->plan.in; }
+const b200_video_info & vcs_out_info (const b200_vcs * h) { return h->plan.frame_out; }
+
+int vcs_comp_launch (b200_vcs * h, int n, const uint8_t *const *in, uint8_t * dst, const b200_video_info & di,
+    const CompStore & S, cudaStream_t stream)
+{
+  if (!vcs_comp_fusable (h) || n < 1 || n > B200_VCS_MAX_BATCH) return B200_ERR_STATE;
+  DeviceGuard g (h->device);
+  if (!g.ok) return B200_ERR_CUDA;
+  VcsBatch b;
+  for (int i = 0; i < n; i++) { b.in[i] = in[i]; b.out[i] = dst; }
+  unsigned long long off[3];
+  int stride[3];
+  for (int k = 0; k < 3; k++) { off[k] = di.offset[k]; stride[k] = di.stride[k]; }
+  return launch_planes_comp (h->planes, b, n, stream, alignment (b.in, n) >= 8, off, stride, S);
+}
+
+}  // namespace b200
+
 extern "C" {
 
 void b200_vcs_config_init (b200_vcs_config * cfg)

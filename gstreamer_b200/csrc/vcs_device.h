@@ -1,6 +1,7 @@
 // gstreamer_b200/csrc/vcs_device.h — device-side view of a convert+scale plan (product code).
 #pragma once
 
+#include <cuda_runtime.h>
 #include <stdint.h>
 
 #include "../../include/b200dsp.h"
@@ -50,5 +51,28 @@ struct VcsBatch {
   const uint8_t *in[B200_VCS_MAX_BATCH];
   uint8_t *out[B200_VCS_MAX_BATCH];
 };
+
+// How the plane-scaling kernels (vcs_planes*.cuh) store an output byte.  NoStore: into the converter's own output frame.
+// CompStore: the compositor's fused route (b200_comp_blend_convert) - item i of the batch is one pad, output byte (x, y)
+// of the launch's plane k goes to byte (x + px[k][i], y + py[k][i]) of the compositor's destination plane, is dropped
+// outside that plane, and is blended like compositor_orc_blend_u8: (d * (256 - a) + s * a) >> 8, or stored at a >= 256.
+struct NoStore { static constexpr bool fused = false; };
+
+struct CompStore {
+  static constexpr bool fused = true;
+  int dw[3], dh[3];                              // destination plane of the launch's plane k: bytes per row, rows
+  int px[3][B200_VCS_MAX_BATCH], py[3][B200_VCS_MAX_BATCH];
+  int alpha[B200_VCS_MAX_BATCH];
+};
+
+// b200_comp_blend_convert's two halves of the converter (vcs.cu): a converter whose plan is plane scaling into a 4:2:0
+// format can store straight into the compositor's destination; vcs_comp_launch runs its plane kernels in their CompStore
+// form for n pads (S indexed by destination plane), frames in[i], destination `dst` laid out as `di`
+bool vcs_comp_fusable (const b200_vcs * h);
+int vcs_device (const b200_vcs * h);
+const b200_video_info & vcs_in_info (const b200_vcs * h);
+const b200_video_info & vcs_out_info (const b200_vcs * h);
+int vcs_comp_launch (b200_vcs * h, int n, const uint8_t *const *in, uint8_t * dst, const b200_video_info & di,
+    const CompStore & S, cudaStream_t stream);
 
 }  // namespace b200

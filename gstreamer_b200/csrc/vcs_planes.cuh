@@ -67,8 +67,8 @@ constexpr int PL_TW = 64, PL_TH = 4;          // output bytes x rows per CTA
 constexpr int PL_STAGE_COLS = 1024;           // staged first-pass bytes per row (vertical first)
 constexpr int PL_STAGE_ROWS = 40;             // staged first-pass rows (horizontal first)
 
-__global__ void __launch_bounds__ (256)
-vcs_planes_kernel (const PlanesParams P, const VcsBatch frames)
+template <class ST>
+__device__ __forceinline__ void planes_body (const PlanesParams & P, const VcsBatch & frames, const ST & S)
 {
   // first-pass results of this CTA's tile, each computed once:
   //   vertical first:   stage[row of the tile][source byte column]   (4 x PL_STAGE_COLS)
@@ -137,7 +137,8 @@ vcs_planes_kernel (const PlanesParams P, const VcsBatch frames)
         v = src[(size_t) (Q.ih == Q.oh ? y : y >> 1) * Q.sstride + (Q.iw == Q.ow ? xb : xb >> 1)];
         break;
     }
-    dst[(size_t) y * Q.dstride + xb] = (uint8_t) v;
+    if constexpr (ST::fused) comp_store<1> (S, plane, frame, dst, Q.dstride, xb, y, {v});
+    else dst[(size_t) y * Q.dstride + xb] = (uint8_t) v;
     return;
   }
 
@@ -208,7 +209,21 @@ vcs_planes_kernel (const PlanesParams P, const VcsBatch frames)
       v = fir_round_u8 (acc);
     }
   }
-  dst[(size_t) y * Q.dstride + xb] = (uint8_t) v;
+  if constexpr (ST::fused) comp_store<1> (S, plane, frame, dst, Q.dstride, xb, y, {v});
+  else dst[(size_t) y * Q.dstride + xb] = (uint8_t) v;
+}
+
+__global__ void __launch_bounds__ (256)
+vcs_planes_kernel (const PlanesParams P, const VcsBatch frames)
+{
+  planes_body (P, frames, NoStore ());
+}
+
+// the CompStore form (b200_comp_blend_convert's fused route)
+__global__ void __launch_bounds__ (256)
+vcs_planes_comp_kernel (const PlanesParams P, const VcsBatch frames, const CompStore S)
+{
+  planes_body (P, frames, S);
 }
 
 // copy / halve planes with word-aligned rows on their own: one thread = one output word, the grid exactly the plane's words
@@ -350,6 +365,45 @@ inline int launch_planes (const PlanesState & st, const VcsBatch & batch, int n,
   }
   const dim3 grid ((wmax + PL_TW - 1) / PL_TW, (hmax + PL_TH - 1) / PL_TH, P.n_planes * n);
   vcs_planes_kernel <<<grid, 256, 0, stream>>> (P, batch);
+  B200_CUDA_TRY (cudaGetLastError ());
+  return B200_OK;
+}
+
+// The same launches in their CompStore form (b200_comp_blend_convert's fused route): plane i stores into the destination
+// plane at dst_off[i] / dstride[i], S indexed by plane.  The copy / halve planes of vcs_planes_vec_kernel take
+// vcs_planes_kernel's byte path here: the fused store clips and blends byte by byte.
+inline int launch_planes_comp (const PlanesState & st, const VcsBatch & batch, int n, cudaStream_t stream, bool aligned,
+    const unsigned long long *dst_off, const int *dstride, const CompStore & S)
+{
+  PlanesParams P;
+  memset (&P, 0, sizeof (P));
+  CompStore SP, SF;                                                // the byte kernel's planes / one word-wide plane
+  memcpy (SP.alpha, S.alpha, sizeof (S.alpha));
+  memcpy (SF.alpha, S.alpha, sizeof (S.alpha));
+  for (int i = 0; i < st.params.n_planes; i++) {
+    CompStore & T = aligned && st.fast[i].ok ? SF : SP;
+    const int k = &T == &SF ? 0 : P.n_planes;
+    T.dw[k] = S.dw[i]; T.dh[k] = S.dh[i];
+    memcpy (T.px[k], S.px[i], sizeof (S.px[i])); memcpy (T.py[k], S.py[i], sizeof (S.py[i]));
+    if (&T == &SF) {
+      PlaneFastState f = st.fast[i];
+      f.dev.dst_off = dst_off[i]; f.dev.dstride = dstride[i];
+      const int s = launch_plane_fast<CompStore> (f, batch, n, stream, SF);
+      if (s != B200_OK) return s;
+    } else {
+      PlaneDev & q = P.pl[P.n_planes++];
+      q = st.params.pl[i];
+      q.dst_off = dst_off[i]; q.dstride = dstride[i]; q.vec4 = 0;
+    }
+  }
+  if (P.n_planes == 0) return B200_OK;
+  int wmax = 0, hmax = 0;
+  for (int i = 0; i < P.n_planes; i++) {
+    wmax = max (wmax, P.pl[i].ow * P.pl[i].ne);
+    hmax = max (hmax, P.pl[i].oh);
+  }
+  const dim3 grid ((wmax + PL_TW - 1) / PL_TW, (hmax + PL_TH - 1) / PL_TH, P.n_planes * n);
+  vcs_planes_comp_kernel <<<grid, 256, 0, stream>>> (P, batch, SP);
   B200_CUDA_TRY (cudaGetLastError ());
   return B200_OK;
 }

@@ -44,6 +44,19 @@ struct PlaneFastDev {
 
 constexpr int PLF_THREADS = 256;
 
+// CompStore form of a plane kernel's store: NC bytes of output pixel byte column xb, row y of the launch's plane k, item i
+// (base = the destination plane's first byte)
+template <int NC> __device__ __forceinline__ void comp_store (const CompStore & S, int k, int i, uint8_t *base, int stride,
+    int xb, int y, const int (&v)[NC])
+{
+  const int X = S.px[k][i] + xb, Y = S.py[k][i] + y;
+  if (X < 0 || X + NC > S.dw[k] || Y < 0 || Y >= S.dh[k]) return;
+  uint8_t *p = base + (size_t) Y * stride + X;
+  const int a = S.alpha[i];
+#pragma unroll
+  for (int c = 0; c < NC; c++) p[c] = (uint8_t) (a >= 256 ? v[c] : (p[c] * (256 - a) + v[c] * a) >> 8);
+}
+
 // the NC words of one pixel column (one per component) as a single shared-memory access
 template <int NC> __device__ __forceinline__ void plf_ld (const unsigned *p, unsigned (&v)[NC])
 {
@@ -60,9 +73,8 @@ template <int NC> __device__ __forceinline__ void plf_st (unsigned *p, const uns
 
 // HM / VM: PassMode of the axis (1 copy / nearest, 2 two taps, 3 n taps); NC: bytes per pixel (1, 2 for interleaved UV, 4 for
 // packed RGB); NTW > 0: every n-tap axis uses exactly NTW packed tap words (straight-line FIRs), 0: run-time loops
-template <int HM, int VM, int NC, int NTW = 0>
-__global__ void __launch_bounds__ (PLF_THREADS, 2)
-vcs_planes_fast_kernel (const PlaneFastDev Q, const VcsBatch frames)
+template <int HM, int VM, int NC, int NTW, class ST>
+__device__ __forceinline__ void planes_fast_body (const PlaneFastDev & Q, const VcsBatch & frames, const ST & S)
 {
   extern __shared__ __align__ (16) unsigned plsm[];
   const int ngr = Q.rows / 4, groups = ngr + 1 + Q.ntw_v;
@@ -211,7 +223,8 @@ vcs_planes_fast_kernel (const PlaneFastDev Q, const VcsBatch frames)
 #pragma unroll
         for (int c = 0; c < NC; c++) v[c] = (int) ((lo[c] >> sh) & 0xffu);
       }
-      if (NC == 1) *dp = (uint8_t) v[0];
+      if constexpr (ST::fused) comp_store<NC> (S, 0, blockIdx.z, dst, Q.dstride, (ox0 + tx) * NC, oy0 + ty, v);
+      else if (NC == 1) *dp = (uint8_t) v[0];
       else if (NC == 2) *(unsigned short *) dp = (unsigned short) ((unsigned) v[0] | ((unsigned) v[1 % NC] << 8));
       else {                                                       // 4-byte pixel, optionally in another byte order (PlaneFastDev::swz)
         const unsigned px = (unsigned) v[0] | ((unsigned) v[1 % NC] << 8) | ((unsigned) v[2 % NC] << 16) | ((unsigned) v[3 % NC] << 24);
@@ -219,6 +232,21 @@ vcs_planes_fast_kernel (const PlaneFastDev Q, const VcsBatch frames)
       }
     }
   }
+}
+
+template <int HM, int VM, int NC, int NTW = 0>
+__global__ void __launch_bounds__ (PLF_THREADS, 2)
+vcs_planes_fast_kernel (const PlaneFastDev Q, const VcsBatch frames)
+{
+  planes_fast_body<HM, VM, NC, NTW> (Q, frames, NoStore ());
+}
+
+// the CompStore form (b200_comp_blend_convert's fused route)
+template <int HM, int VM, int NC, int NTW = 0>
+__global__ void __launch_bounds__ (PLF_THREADS, 2)
+vcs_planes_fast_comp_kernel (const PlaneFastDev Q, const VcsBatch frames, const CompStore S)
+{
+  planes_fast_body<HM, VM, NC, NTW> (Q, frames, S);
 }
 
 // ---- vertical pass first (gst_video_scaler_2d picks it whenever the plane shrinks vertically, video-scaler.c:1515-1520) -----------
@@ -229,9 +257,8 @@ vcs_planes_fast_kernel (const PlaneFastDev Q, const VcsBatch frames)
 //  C' the horizontal pass: a thread owns one output byte (or U,V pair): funnel shift to the window's first pixel, IDP.4A / lerp /
 //     byte select on the v-scaled row, one store, lanes on consecutive columns.
 // NTW > 0: every n-tap axis of the plane uses exactly NTW packed tap words (straight-line FIRs); 0: run-time loops
-template <int HM, int VM, int NC, int NTW = 0>
-__global__ void __launch_bounds__ (PLF_THREADS, 2)
-vcs_planes_fast_vfirst_kernel (const PlaneFastDev Q, const VcsBatch frames)
+template <int HM, int VM, int NC, int NTW, class ST>
+__device__ __forceinline__ void planes_fast_vfirst_body (const PlaneFastDev & Q, const VcsBatch & frames, const ST & S)
 {
   extern __shared__ __align__ (16) unsigned plsm[];
   const int ngr = Q.rows / 4;
@@ -372,7 +399,8 @@ vcs_planes_fast_vfirst_kernel (const PlaneFastDev Q, const VcsBatch frames)
           v[c] = (int) ((tp[0] >> sh) & 0xffu);
         }
       }
-      if (NC == 1) *dp = (uint8_t) v[0];
+      if constexpr (ST::fused) comp_store<NC> (S, 0, blockIdx.z, dst, Q.dstride, (ox0 + tx) * NC, oy0 + ty, v);
+      else if (NC == 1) *dp = (uint8_t) v[0];
       else if (NC == 2) *(unsigned short *) dp = (unsigned short) ((unsigned) v[0] | ((unsigned) v[1 % NC] << 8));
       else {                                                       // 4-byte pixel, optionally in another byte order (PlaneFastDev::swz)
         const unsigned px = (unsigned) v[0] | ((unsigned) v[1 % NC] << 8) | ((unsigned) v[2 % NC] << 16) | ((unsigned) v[3 % NC] << 24);
@@ -380,6 +408,21 @@ vcs_planes_fast_vfirst_kernel (const PlaneFastDev Q, const VcsBatch frames)
       }
     }
   }
+}
+
+template <int HM, int VM, int NC, int NTW = 0>
+__global__ void __launch_bounds__ (PLF_THREADS, 2)
+vcs_planes_fast_vfirst_kernel (const PlaneFastDev Q, const VcsBatch frames)
+{
+  planes_fast_vfirst_body<HM, VM, NC, NTW> (Q, frames, NoStore ());
+}
+
+// the CompStore form (b200_comp_blend_convert's fused route)
+template <int HM, int VM, int NC, int NTW = 0>
+__global__ void __launch_bounds__ (PLF_THREADS, 2)
+vcs_planes_fast_vfirst_comp_kernel (const PlaneFastDev Q, const VcsBatch frames, const CompStore S)
+{
+  planes_fast_vfirst_body<HM, VM, NC, NTW> (Q, frames, S);
 }
 
 // ------------------------------------------------------------------------------------ host side
@@ -395,21 +438,37 @@ struct PlaneFastState {
   int *d_hp = nullptr, *d_vp = nullptr;
 };
 
-typedef void (*plane_fast_fn) (const PlaneFastDev, const VcsBatch);
+template <class ST> struct PlaneFastFn { using type = void (*) (const PlaneFastDev, const VcsBatch, const CompStore); };
+template <> struct PlaneFastFn<NoStore> { using type = void (*) (const PlaneFastDev, const VcsBatch); };
+template <class ST = NoStore> using plane_fast_fn = typename PlaneFastFn<ST>::type;
 
-inline plane_fast_fn plane_fast_kernel_for (int hm, int vm, int nc, bool vfirst, int ntw = 0)
+// the kernel of a store form: vcs_planes_fast[_vfirst]_kernel, or its CompStore form
+template <class ST, bool VFIRST, int H, int V, int NC, int NTW> constexpr plane_fast_fn<ST> plf_kernel ()
+{
+  if constexpr (ST::fused && VFIRST) return vcs_planes_fast_vfirst_comp_kernel<H, V, NC, NTW>;
+  else if constexpr (ST::fused) return vcs_planes_fast_comp_kernel<H, V, NC, NTW>;
+  else if constexpr (VFIRST) return vcs_planes_fast_vfirst_kernel<H, V, NC, NTW>;
+  else return vcs_planes_fast_kernel<H, V, NC, NTW>;
+}
+
+// the instantiation a plane runs; the CompStore forms exist for the 1- and 2-byte pixels of 4:2:0 planes only
+template <class ST = NoStore>
+inline plane_fast_fn<ST> plane_fast_kernel_for (int hm, int vm, int nc, bool vfirst, int ntw = 0)
 {
 #define PLF_PICK(H, V)                                                                         \
   if (hm == H && vm == V) {                                                                    \
-    if (nc == 4 && vfirst && ntw == 2 && (H == 3 || V == 3)) return vcs_planes_fast_vfirst_kernel<H, V, 4, 2>;   \
-    if (nc == 4 && !vfirst && ntw == 2 && (H == 3 || V == 3)) return vcs_planes_fast_kernel<H, V, 4, 2>;   \
-    if (nc == 4 && !vfirst && ntw == 1 && (H == 3 || V == 3)) return vcs_planes_fast_kernel<H, V, 4, 1>;   \
-    if (nc != 4 && !vfirst && ntw == 1 && (H == 3 || V == 3)) return nc == 1 ? vcs_planes_fast_kernel<H, V, 1, 1> : vcs_planes_fast_kernel<H, V, 2, 1>;   \
-    if (nc == 4) return vfirst ? vcs_planes_fast_vfirst_kernel<H, V, 4> : vcs_planes_fast_kernel<H, V, 4>;   \
-    if (vfirst && ntw == 2 && (H == 3 || V == 3)) return nc == 1 ? vcs_planes_fast_vfirst_kernel<H, V, 1, 2> : vcs_planes_fast_vfirst_kernel<H, V, 2, 2>;   \
-    if (vfirst && ntw == 1 && (H == 3 || V == 3)) return nc == 1 ? vcs_planes_fast_vfirst_kernel<H, V, 1, 1> : vcs_planes_fast_vfirst_kernel<H, V, 2, 1>;   \
-    if (vfirst) return nc == 1 ? vcs_planes_fast_vfirst_kernel<H, V, 1> : vcs_planes_fast_vfirst_kernel<H, V, 2>;   \
-    return nc == 1 ? vcs_planes_fast_kernel<H, V, 1> : vcs_planes_fast_kernel<H, V, 2>;       \
+    if constexpr (!ST::fused) {                                                                \
+      if (nc == 4 && vfirst && ntw == 2 && (H == 3 || V == 3)) return vcs_planes_fast_vfirst_kernel<H, V, 4, 2>;   \
+      if (nc == 4 && !vfirst && ntw == 2 && (H == 3 || V == 3)) return vcs_planes_fast_kernel<H, V, 4, 2>;   \
+      if (nc == 4 && !vfirst && ntw == 1 && (H == 3 || V == 3)) return vcs_planes_fast_kernel<H, V, 4, 1>;   \
+      if (nc == 4) return vfirst ? vcs_planes_fast_vfirst_kernel<H, V, 4> : vcs_planes_fast_kernel<H, V, 4>;   \
+    }                                                                                          \
+    if (nc == 4) return nullptr;                                                               \
+    if (!vfirst && ntw == 1 && (H == 3 || V == 3)) return nc == 1 ? plf_kernel<ST, false, H, V, 1, 1> () : plf_kernel<ST, false, H, V, 2, 1> ();   \
+    if (vfirst && ntw == 2 && (H == 3 || V == 3)) return nc == 1 ? plf_kernel<ST, true, H, V, 1, 2> () : plf_kernel<ST, true, H, V, 2, 2> ();   \
+    if (vfirst && ntw == 1 && (H == 3 || V == 3)) return nc == 1 ? plf_kernel<ST, true, H, V, 1, 1> () : plf_kernel<ST, true, H, V, 2, 1> ();   \
+    if (vfirst) return nc == 1 ? plf_kernel<ST, true, H, V, 1, 0> () : plf_kernel<ST, true, H, V, 2, 0> ();   \
+    return nc == 1 ? plf_kernel<ST, false, H, V, 1, 0> () : plf_kernel<ST, false, H, V, 2, 0> ();       \
   }
   PLF_PICK (1, 1) PLF_PICK (1, 2) PLF_PICK (1, 3) PLF_PICK (2, 1) PLF_PICK (2, 2) PLF_PICK (2, 3)
   PLF_PICK (3, 1) PLF_PICK (3, 2) PLF_PICK (3, 3)
@@ -525,6 +584,8 @@ inline int prepare_plane_fast (const PlanePlan & q, const std::vector<int32_t> &
   if ((s = upload (&st->d_vp, vp.data (), vp.size ())) != B200_OK) return s;
   st->dev.hoff = st->d_hoff; st->dev.voff = st->d_voff; st->dev.hcoef = st->d_hcoef; st->dev.vcoef = st->d_vcoef;
   st->dev.h_packed = st->d_hp; st->dev.v_packed = st->d_vp;
+  if (st->nc != 4 && (s = allow_max_dyn_smem (plane_fast_kernel_for<CompStore> (st->hm, st->vm, st->nc, st->vfirst, st->ntw))) != B200_OK)
+    return s;
   return allow_max_dyn_smem (plane_fast_kernel_for (st->hm, st->vm, st->nc, st->vfirst, st->ntw));
 }
 
@@ -533,12 +594,14 @@ inline void free_plane_fast (PlaneFastState * st)
   cudaFree (st->d_hoff); cudaFree (st->d_voff); cudaFree (st->d_hcoef); cudaFree (st->d_vcoef); cudaFree (st->d_hp); cudaFree (st->d_vp);
 }
 
-inline int launch_plane_fast (const PlaneFastState & st, const VcsBatch & batch, int n, cudaStream_t stream)
+template <class ST = NoStore>
+inline int launch_plane_fast (const PlaneFastState & st, const VcsBatch & batch, int n, cudaStream_t stream, const ST & S = ST ())
 {
-  plane_fast_fn fn = plane_fast_kernel_for (st.hm, st.vm, st.nc, st.vfirst, st.ntw);
+  plane_fast_fn<ST> fn = plane_fast_kernel_for<ST> (st.hm, st.vm, st.nc, st.vfirst, st.ntw);
   if (!fn) return B200_ERR_STATE;
   const dim3 grid ((st.dev.ow + st.dev.tw - 1) / st.dev.tw, (st.dev.oh + st.dev.th - 1) / st.dev.th, n);
-  fn <<<grid, PLF_THREADS, st.smem, stream>>> (st.dev, batch);
+  if constexpr (ST::fused) fn <<<grid, PLF_THREADS, st.smem, stream>>> (st.dev, batch, S);
+  else fn <<<grid, PLF_THREADS, st.smem, stream>>> (st.dev, batch);
   B200_CUDA_TRY (cudaGetLastError ());
   return B200_OK;
 }

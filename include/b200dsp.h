@@ -276,6 +276,28 @@ int b200_comp_blend_yuv_host_submit (b200_comp * h, void *dst_host, const b200_v
 int b200_comp_blend_yuv_host (b200_comp * h, void *dst_host, const b200_video_info * dst_info, int background,
     const b200_comp_pad_yuv * pads, int n_pads);
 
+/* Convert pads (GstVideoAggregatorConvertPad, gstvideoaggregator.c:479-640): a pad whose caps differ from the output's
+ * carries the converter from its caps to the output format at the pad's output size.  The caller creates it with
+ * b200_vcs_create: B200_SCALE_MITCHELL (the converter's default cubic), no destination rectangle, the output's colour
+ * matrix, range and chroma site, and the pad's frame layout as input; pads with equal conversions may share one. */
+typedef struct {
+  const void *data;              /* device pointer to the pad's frame */
+  b200_video_info info;          /* the pad's caps and plane layout (with conv: the input conv was created with) */
+  b200_vcs *conv;                /* NULL: the frame already has the output's format; the pad is info.width x info.height */
+  int32_t xpos, ypos;            /* sizing-policy offsets included */
+  double alpha;
+  int32_t op;                    /* b200_comp_operator */
+  int32_t reserved;
+} b200_comp_pad_convert;
+/* b200_comp_blend / b200_comp_blend_yuv with convert pads, in z-order, for the packed RGBA family and I420 / YV12 / NV12 / NV21
+ * (other outputs: conv == NULL pads only).  Pads with alpha 0 are dropped before any conversion.  A 4:2:0 output's pads
+ * whose converter scales planes (same 4:2:0 format) are scaled straight into dst; other converted pads go through a
+ * converted frame the handle owns, so calls on one handle must be issued on one stream (or be ordered by the caller).
+ * Every converter must live on the handle's device.  dst_info: the destination's format (the handle's), size and layout.
+ * Device memory. */
+int b200_comp_blend_convert (b200_comp * h, void *dst, const b200_video_info * dst_info, int background,
+    const b200_comp_pad_convert * pads, int n_pads, void *cuda_stream);
+
 /* ------------------------------------------------------------------ audio resampler */
 typedef struct b200_ars b200_ars;
 /* GstAudioFormat values (gst-libs/gst/audio/audio-format.h:97-140) of the sample formats audioresample hands to
