@@ -1767,16 +1767,9 @@ struct b200_ars {
   // reference state (audio-resampler-private.h:103-112)
   int samp_index = 0, samp_phase = 0, skip = 0;
   size_t samples_avail = 0;
-  // system-memory peers (b200_ars_process_host*): ring of device staging slots, upload / kernels / download on three streams
+  // system-memory peers (b200_ars_process_host*)
   static const int kSlots = 3;
-  struct HostSlot {
-    uint8_t *d_in = nullptr, *d_out = nullptr;
-    size_t in_cap = 0, out_cap = 0;
-    cudaEvent_t ev_in = nullptr, ev_run = nullptr, ev_out = nullptr;
-    bool used = false;
-  } slot[kSlots];
-  cudaStream_t s_h2d = nullptr, s_run = nullptr, s_d2h = nullptr;
-  unsigned long long submitted = 0;
+  HostRing<kSlots> ring;
 };
 
 static int ars_reset_state (b200_ars * h, cudaStream_t stream)
@@ -1888,16 +1881,8 @@ void b200_ars_destroy (b200_ars * h)
   if (h->device >= 0) {
     DeviceGuard g (h->device);
     cudaFree (h->d_phases); cudaFree (h->d_qtab); cudaFree (h->d_proto); cudaFree (h->d_table_x); cudaFree (h->d_hist[0]); cudaFree (h->d_hist[1]);
-    if (h->s_h2d) {
-      cudaStreamSynchronize (h->s_d2h);
-      for (int i = 0; i < b200_ars::kSlots; i++) {
-        cudaFree (h->slot[i].d_in); cudaFree (h->slot[i].d_out);
-        if (h->slot[i].ev_in) cudaEventDestroy (h->slot[i].ev_in);
-        if (h->slot[i].ev_run) cudaEventDestroy (h->slot[i].ev_run);
-        if (h->slot[i].ev_out) cudaEventDestroy (h->slot[i].ev_out);
-      }
-      cudaStreamDestroy (h->s_h2d); cudaStreamDestroy (h->s_run); cudaStreamDestroy (h->s_d2h);
-    }
+    h->ring.drain ();
+    h->ring.release ();
   }
   delete h;
 }
@@ -2178,50 +2163,22 @@ int b200_ars_process_host_submit (b200_ars * h, const void *in_host, size_t in_f
   if (h->device < 0) return B200_ERR_NO_DEVICE;
   DeviceGuard g (h->device);
   if (!g.ok) return B200_ERR_CUDA;
-  if (!h->s_h2d) {
-    B200_CUDA_TRY (cudaStreamCreateWithFlags (&h->s_h2d, cudaStreamNonBlocking));
-    B200_CUDA_TRY (cudaStreamCreateWithFlags (&h->s_run, cudaStreamNonBlocking));
-    B200_CUDA_TRY (cudaStreamCreateWithFlags (&h->s_d2h, cudaStreamNonBlocking));
-    for (int i = 0; i < b200_ars::kSlots; i++) {
-      B200_CUDA_TRY (cudaEventCreateWithFlags (&h->slot[i].ev_in, cudaEventDisableTiming));
-      B200_CUDA_TRY (cudaEventCreateWithFlags (&h->slot[i].ev_run, cudaEventDisableTiming));
-      B200_CUDA_TRY (cudaEventCreateWithFlags (&h->slot[i].ev_out, cudaEventDisableTiming));
-    }
-  }
-  b200_ars::HostSlot & sl = h->slot[h->submitted % b200_ars::kSlots];
+  B200_CUDA_TRY (h->ring.setup ());
   const size_t bpf = (size_t) h->plan.channels * h->plan.bps;
   const size_t in_bytes = in_host ? in_frames * bpf : 0;
   const size_t want = b200_ars_get_out_frames (h, in_frames);
   if (want > out_capacity_frames) return B200_ERR_INVALID_ARG;
   const size_t out_bytes = want * bpf;
-  if (sl.used) {
-    B200_CUDA_TRY (cudaStreamWaitEvent (h->s_h2d, sl.ev_run, 0));   // the slot's previous kernels have read its input
-    B200_CUDA_TRY (cudaStreamWaitEvent (h->s_run, sl.ev_out, 0));   // ... and its output has been downloaded
-  }
-  if (in_bytes > sl.in_cap) {
-    if (sl.used) B200_CUDA_TRY (cudaEventSynchronize (sl.ev_run));
-    B200_CUDA_TRY (cudaFree (sl.d_in)); sl.d_in = nullptr; sl.in_cap = 0;
-    B200_CUDA_TRY (cudaMalloc ((void **) &sl.d_in, in_bytes + in_bytes / 4));
-    sl.in_cap = in_bytes + in_bytes / 4;
-  }
-  if (out_bytes > sl.out_cap) {
-    if (sl.used) B200_CUDA_TRY (cudaEventSynchronize (sl.ev_out));
-    B200_CUDA_TRY (cudaFree (sl.d_out)); sl.d_out = nullptr; sl.out_cap = 0;
-    B200_CUDA_TRY (cudaMalloc ((void **) &sl.d_out, out_bytes + out_bytes / 4));
-    sl.out_cap = out_bytes + out_bytes / 4;
-  }
-  if (in_bytes) B200_CUDA_TRY (cudaMemcpyAsync (sl.d_in, in_host, in_bytes, cudaMemcpyHostToDevice, h->s_h2d));
-  B200_CUDA_TRY (cudaEventRecord (sl.ev_in, h->s_h2d));
-  B200_CUDA_TRY (cudaStreamWaitEvent (h->s_run, sl.ev_in, 0));
+  auto & r = h->ring;
+  B200_CUDA_TRY (r.take (in_bytes, in_bytes + in_bytes / 4, out_bytes, out_bytes + out_bytes / 4));
+  if (in_bytes) B200_CUDA_TRY (r.upload (r.in (), in_host, in_bytes));
+  B200_CUDA_TRY (r.inputs_ready ());
   size_t got = 0;
-  int st = b200_ars_process (h, in_host ? sl.d_in : nullptr, in_frames, sl.d_out, want, &got, h->s_run);
+  int st = b200_ars_process (h, in_host ? r.in () : nullptr, in_frames, r.out (), want, &got, r.run_stream ());
   if (st != B200_OK) return st;
-  B200_CUDA_TRY (cudaEventRecord (sl.ev_run, h->s_run));
-  B200_CUDA_TRY (cudaStreamWaitEvent (h->s_d2h, sl.ev_run, 0));
-  if (got) B200_CUDA_TRY (cudaMemcpyAsync (out_host, sl.d_out, got * bpf, cudaMemcpyDeviceToHost, h->s_d2h));
-  B200_CUDA_TRY (cudaEventRecord (sl.ev_out, h->s_d2h));
-  sl.used = true;
-  h->submitted++;
+  B200_CUDA_TRY (r.run_done ());
+  if (got) B200_CUDA_TRY (r.download (out_host, r.out (), got * bpf));
+  B200_CUDA_TRY (r.finish ());
   if (out_frames) *out_frames = got;
   return B200_OK;
 }
@@ -2230,11 +2187,10 @@ int b200_ars_process_host_wait (b200_ars * h, int keep_in_flight)
 {
   if (!h || keep_in_flight < 0 || keep_in_flight >= b200_ars::kSlots) return B200_ERR_INVALID_ARG;
   if (h->device < 0) return B200_ERR_NO_DEVICE;
-  if (!h->s_h2d || h->submitted <= (unsigned long long) keep_in_flight) return B200_OK;
+  if (h->ring.idle (keep_in_flight)) return B200_OK;
   DeviceGuard g (h->device);
   if (!g.ok) return B200_ERR_CUDA;
-  const unsigned long long last = h->submitted - 1 - (unsigned long long) keep_in_flight;
-  B200_CUDA_TRY (cudaEventSynchronize (h->slot[last % b200_ars::kSlots].ev_out));
+  B200_CUDA_TRY (h->ring.wait (keep_in_flight));
   return B200_OK;
 }
 

@@ -336,22 +336,12 @@ comp_yuv_kernel (const CompYuvParams P)
 
 using namespace b200;
 
-// system-memory peers (b200_comp_blend_host*): a ring of device slots, each holding the staged pads and the destination
-// of one output frame; uploads, the blend and the download of consecutive frames run on three streams and overlap
-struct CompHostSlot {
-  uint8_t *d_pads = nullptr, *d_dst = nullptr;
-  size_t pads_cap = 0, dst_cap = 0;
-  cudaEvent_t ev_in = nullptr, ev_run = nullptr, ev_out = nullptr;
-  bool used = false;
-};
-
 struct b200_comp {
   int format, width, height, device;
   int alpha_shift;
+  // system-memory peers (b200_comp_blend_host*): each slot holds the staged pads (in) and the destination (out) of one frame
   static const int kSlots = 3;
-  CompHostSlot slot[kSlots];
-  cudaStream_t s_h2d = nullptr, s_run = nullptr, s_d2h = nullptr;
-  unsigned long long submitted = 0;
+  HostRing<kSlots> ring;
   uint8_t *d_conv = nullptr;     // b200_comp_blend_convert: the two-pass pads' converted frames
   size_t conv_cap = 0;
 };
@@ -485,6 +475,36 @@ PadRoute pad_route (const b200_vcs * conv, bool yuv420_out, int blend_alpha, boo
   return PR_TWO_PASS;                                              // b200_vcs_convert_batch into d_conv, then the blend kernel
 }
 
+// The staging both host entry points share: pad i's `bytes[i]` get a 256-byte aligned place in the slot's pad buffer
+// and travel up where `up[i]`; `blend` runs on the run stream over the pads' device copies; the destination comes back
+// (and with `dst_up` first travels up).  The entry points have checked the arguments and set the ring up.
+template <typename Pad, typename Blend>
+static int comp_host_submit (b200_comp * h, void *dst_host, size_t dst_bytes, bool dst_up, const Pad * pads, int n_pads,
+    const size_t * bytes, const bool * up, Blend blend)
+{
+  size_t need = 0, off[B200_COMP_MAX_PADS];
+  for (int i = 0; i < n_pads; i++) {
+    off[i] = need;
+    need += (bytes[i] + 255) & ~(size_t) 255;
+  }
+  auto & r = h->ring;
+  B200_CUDA_TRY (r.take (need, need, dst_bytes, dst_bytes));
+  Pad dev_pads[B200_COMP_MAX_PADS];
+  for (int i = 0; i < n_pads; i++) {
+    dev_pads[i] = pads[i];
+    dev_pads[i].data = r.in () + off[i];
+    if (up[i]) B200_CUDA_TRY (r.upload (r.in () + off[i], pads[i].data, bytes[i]));
+  }
+  B200_CUDA_TRY (r.inputs_ready ());
+  if (dst_up) B200_CUDA_TRY (cudaMemcpyAsync (r.out (), dst_host, dst_bytes, cudaMemcpyHostToDevice, r.run_stream ()));
+  const int st = blend (r.out (), dev_pads, r.run_stream ());
+  if (st != B200_OK) return st;
+  B200_CUDA_TRY (r.run_done ());
+  B200_CUDA_TRY (r.download (dst_host, r.out (), dst_bytes));
+  B200_CUDA_TRY (r.finish ());
+  return B200_OK;
+}
+
 extern "C" {
 
 int b200_comp_create (int out_format, int width, int height, int device, b200_comp ** handle)
@@ -514,21 +534,11 @@ int b200_comp_create (int out_format, int width, int height, int device, b200_co
 void b200_comp_destroy (b200_comp * h)
 {
   if (!h) return;
-  if (h->device >= 0 && h->s_h2d) {
+  if (h->device >= 0) {
     DeviceGuard g (h->device);
-    cudaStreamSynchronize (h->s_d2h);
-    for (int i = 0; i < b200_comp::kSlots; i++) {
-      CompHostSlot & sl = h->slot[i];
-      cudaFree (sl.d_pads); cudaFree (sl.d_dst);
-      if (sl.ev_in) cudaEventDestroy (sl.ev_in);
-      if (sl.ev_run) cudaEventDestroy (sl.ev_run);
-      if (sl.ev_out) cudaEventDestroy (sl.ev_out);
-    }
-    cudaStreamDestroy (h->s_h2d); cudaStreamDestroy (h->s_run); cudaStreamDestroy (h->s_d2h);
-  }
-  if (h->device >= 0 && h->d_conv) {
-    DeviceGuard g (h->device);
-    cudaFree (h->d_conv);
+    h->ring.drain ();
+    h->ring.release ();
+    if (h->d_conv) cudaFree (h->d_conv);
   }
   delete h;
 }
@@ -743,20 +753,6 @@ int b200_comp_blend_convert (b200_comp * h, void *dst, const b200_video_info * d
   return B.finish ();
 }
 
-static int comp_host_ready (b200_comp * h)
-{
-  if (h->s_h2d) return B200_OK;
-  B200_CUDA_TRY (cudaStreamCreateWithFlags (&h->s_h2d, cudaStreamNonBlocking));
-  B200_CUDA_TRY (cudaStreamCreateWithFlags (&h->s_run, cudaStreamNonBlocking));
-  B200_CUDA_TRY (cudaStreamCreateWithFlags (&h->s_d2h, cudaStreamNonBlocking));
-  for (int i = 0; i < b200_comp::kSlots; i++) {
-    B200_CUDA_TRY (cudaEventCreateWithFlags (&h->slot[i].ev_in, cudaEventDisableTiming));
-    B200_CUDA_TRY (cudaEventCreateWithFlags (&h->slot[i].ev_run, cudaEventDisableTiming));
-    B200_CUDA_TRY (cudaEventCreateWithFlags (&h->slot[i].ev_out, cudaEventDisableTiming));
-  }
-  return B200_OK;
-}
-
 int b200_comp_blend_host_submit (b200_comp * h, void *dst_host, int32_t dst_stride, int background,
     const b200_comp_pad * pads, int n_pads)
 {
@@ -766,64 +762,30 @@ int b200_comp_blend_host_submit (b200_comp * h, void *dst_host, int32_t dst_stri
   if (h->device < 0) return B200_ERR_NO_DEVICE;
   DeviceGuard g (h->device);
   if (!g.ok) return B200_ERR_CUDA;
-  int st = comp_host_ready (h);
-  if (st != B200_OK) return st;
-  CompHostSlot & sl = h->slot[h->submitted % b200_comp::kSlots];
-  // staged layout: the pads one after another (each 256-byte aligned), rows at the caller's stride
-  size_t need = 0, off[B200_COMP_MAX_PADS];
+  B200_CUDA_TRY (h->ring.setup ());
+  // staged layout: rows at the caller's stride
+  size_t bytes[B200_COMP_MAX_PADS];
+  bool up[B200_COMP_MAX_PADS];
   for (int i = 0; i < n_pads; i++) {
     if (!pads[i].data || pads[i].width < 1 || pads[i].height < 1 || pads[i].stride < pads[i].width * 4) return B200_ERR_INVALID_ARG;
-    off[i] = need;
-    need += ((size_t) pads[i].stride * pads[i].height + 255) & ~(size_t) 255;
+    bytes[i] = (size_t) pads[i].stride * pads[i].height;
+    up[i] = !(pads[i].alpha <= 0.0 && pads[i].op != B200_COMP_OP_SOURCE);       // else never read by the blend
   }
-  const size_t dst_bytes = (size_t) dst_stride * h->height;
-  if (sl.used) {                                                   // the slot's previous frame: its blend read the pads, its download read the dst
-    B200_CUDA_TRY (cudaStreamWaitEvent (h->s_h2d, sl.ev_run, 0));
-    B200_CUDA_TRY (cudaStreamWaitEvent (h->s_run, sl.ev_out, 0));
-  }
-  if (need > sl.pads_cap) {
-    if (sl.used) B200_CUDA_TRY (cudaEventSynchronize (sl.ev_run));
-    B200_CUDA_TRY (cudaFree (sl.d_pads)); sl.d_pads = nullptr; sl.pads_cap = 0;
-    B200_CUDA_TRY (cudaMalloc ((void **) &sl.d_pads, need));
-    sl.pads_cap = need;
-  }
-  if (dst_bytes > sl.dst_cap) {
-    if (sl.used) B200_CUDA_TRY (cudaEventSynchronize (sl.ev_out));
-    B200_CUDA_TRY (cudaFree (sl.d_dst)); sl.d_dst = nullptr; sl.dst_cap = 0;
-    B200_CUDA_TRY (cudaMalloc ((void **) &sl.d_dst, dst_bytes));
-    sl.dst_cap = dst_bytes;
-  }
-  b200_comp_pad dev_pads[B200_COMP_MAX_PADS];
-  for (int i = 0; i < n_pads; i++) {
-    dev_pads[i] = pads[i];
-    dev_pads[i].data = sl.d_pads + off[i];
-    if (pads[i].alpha <= 0.0 && pads[i].op != B200_COMP_OP_SOURCE) continue;       // never read by the blend
-    B200_CUDA_TRY (cudaMemcpyAsync (sl.d_pads + off[i], pads[i].data, (size_t) pads[i].stride * pads[i].height,
-            cudaMemcpyHostToDevice, h->s_h2d));
-  }
-  B200_CUDA_TRY (cudaEventRecord (sl.ev_in, h->s_h2d));
-  B200_CUDA_TRY (cudaStreamWaitEvent (h->s_run, sl.ev_in, 0));
-  if ((st = b200_comp_blend (h, sl.d_dst, dst_stride, background, dev_pads, n_pads, h->s_run)) != B200_OK) return st;
-  B200_CUDA_TRY (cudaEventRecord (sl.ev_run, h->s_run));
-  B200_CUDA_TRY (cudaStreamWaitEvent (h->s_d2h, sl.ev_run, 0));
-  B200_CUDA_TRY (cudaMemcpyAsync (dst_host, sl.d_dst, dst_bytes, cudaMemcpyDeviceToHost, h->s_d2h));
-  B200_CUDA_TRY (cudaEventRecord (sl.ev_out, h->s_d2h));
-  sl.used = true;
-  h->submitted++;
-  return B200_OK;
+  return comp_host_submit (h, dst_host, (size_t) dst_stride * h->height, false, pads, n_pads, bytes, up,
+      [&] (uint8_t *dst, const b200_comp_pad *dev_pads, cudaStream_t s) {
+        return b200_comp_blend (h, dst, dst_stride, background, dev_pads, n_pads, s);
+      });
 }
 
 int b200_comp_blend_host_wait (b200_comp * h, int keep_in_flight)
 {
   if (!h || keep_in_flight < 0) return B200_ERR_INVALID_ARG;
   if (h->device < 0) return B200_ERR_NO_DEVICE;
-  if (!h->s_h2d || h->submitted <= (unsigned long long) keep_in_flight) return B200_OK;
+  if (h->ring.idle (keep_in_flight)) return B200_OK;
   DeviceGuard g (h->device);
   if (!g.ok) return B200_ERR_CUDA;
   if (keep_in_flight >= b200_comp::kSlots) return B200_ERR_INVALID_ARG;
-  // the download events complete in submission order: waiting for frame (submitted - 1 - keep) covers all older ones
-  const unsigned long long last = h->submitted - 1 - (unsigned long long) keep_in_flight;
-  B200_CUDA_TRY (cudaEventSynchronize (h->slot[last % b200_comp::kSlots].ev_out));
+  B200_CUDA_TRY (h->ring.wait (keep_in_flight));
   return B200_OK;
 }
 
@@ -845,53 +807,20 @@ int b200_comp_blend_yuv_host_submit (b200_comp * h, void *dst_host, const b200_v
   if (h->device < 0) return B200_ERR_NO_DEVICE;
   DeviceGuard g (h->device);
   if (!g.ok) return B200_ERR_CUDA;
-  int st = comp_host_ready (h);
-  if (st != B200_OK) return st;
-  CompHostSlot & sl = h->slot[h->submitted % b200_comp::kSlots];
-  size_t need = 0, off[B200_COMP_MAX_PADS], bytes[B200_COMP_MAX_PADS];
+  B200_CUDA_TRY (h->ring.setup ());
+  size_t bytes[B200_COMP_MAX_PADS];
+  bool up[B200_COMP_MAX_PADS];
   for (int i = 0; i < n_pads; i++) {
     if (!pads[i].data || pads[i].info.width < 1 || pads[i].info.height < 1) return B200_ERR_INVALID_ARG;
     bytes[i] = b200_video_info_size (&pads[i].info);
-    off[i] = need;
-    need += (bytes[i] + 255) & ~(size_t) 255;
+    up[i] = !(pads[i].alpha == 0.0 && pads[i].op != B200_COMP_OP_SOURCE);       // else never read by the blend
   }
-  const size_t dst_bytes = b200_video_info_size (di);
-  if (sl.used) {
-    B200_CUDA_TRY (cudaStreamWaitEvent (h->s_h2d, sl.ev_run, 0));
-    B200_CUDA_TRY (cudaStreamWaitEvent (h->s_run, sl.ev_out, 0));
-  }
-  if (need > sl.pads_cap) {
-    if (sl.used) B200_CUDA_TRY (cudaEventSynchronize (sl.ev_run));
-    B200_CUDA_TRY (cudaFree (sl.d_pads)); sl.d_pads = nullptr; sl.pads_cap = 0;
-    B200_CUDA_TRY (cudaMalloc ((void **) &sl.d_pads, need));
-    sl.pads_cap = need;
-  }
-  if (dst_bytes > sl.dst_cap) {
-    if (sl.used) B200_CUDA_TRY (cudaEventSynchronize (sl.ev_out));
-    B200_CUDA_TRY (cudaFree (sl.d_dst)); sl.d_dst = nullptr; sl.dst_cap = 0;
-    B200_CUDA_TRY (cudaMalloc ((void **) &sl.d_dst, dst_bytes));
-    sl.dst_cap = dst_bytes;
-  }
-  b200_comp_pad_yuv dev_pads[B200_COMP_MAX_PADS];
-  for (int i = 0; i < n_pads; i++) {
-    dev_pads[i] = pads[i];
-    dev_pads[i].data = sl.d_pads + off[i];
-    if (pads[i].alpha == 0.0 && pads[i].op != B200_COMP_OP_SOURCE) continue;        // never read by the blend
-    B200_CUDA_TRY (cudaMemcpyAsync (sl.d_pads + off[i], pads[i].data, bytes[i], cudaMemcpyHostToDevice, h->s_h2d));
-  }
-  B200_CUDA_TRY (cudaEventRecord (sl.ev_in, h->s_h2d));
-  B200_CUDA_TRY (cudaStreamWaitEvent (h->s_run, sl.ev_in, 0));
   // the blend writes the visible bytes of every plane row only; the rows' stride padding must come back as the caller had it
   // (the reference never touches it), so the destination travels up first
-  B200_CUDA_TRY (cudaMemcpyAsync (sl.d_dst, dst_host, dst_bytes, cudaMemcpyHostToDevice, h->s_run));
-  if ((st = b200_comp_blend_yuv (h, sl.d_dst, di, background, dev_pads, n_pads, h->s_run)) != B200_OK) return st;
-  B200_CUDA_TRY (cudaEventRecord (sl.ev_run, h->s_run));
-  B200_CUDA_TRY (cudaStreamWaitEvent (h->s_d2h, sl.ev_run, 0));
-  B200_CUDA_TRY (cudaMemcpyAsync (dst_host, sl.d_dst, dst_bytes, cudaMemcpyDeviceToHost, h->s_d2h));
-  B200_CUDA_TRY (cudaEventRecord (sl.ev_out, h->s_d2h));
-  sl.used = true;
-  h->submitted++;
-  return B200_OK;
+  return comp_host_submit (h, dst_host, b200_video_info_size (di), true, pads, n_pads, bytes, up,
+      [&] (uint8_t *dst, const b200_comp_pad_yuv *dev_pads, cudaStream_t s) {
+        return b200_comp_blend_yuv (h, dst, di, background, dev_pads, n_pads, s);
+      });
 }
 
 int b200_comp_blend_yuv_host (b200_comp * h, void *dst_host, const b200_video_info * di, int background,

@@ -51,10 +51,7 @@ struct b200_vcs {
   uint8_t *d_cmode = nullptr;
   // host<->device pipeline for system-memory peers
   static const int kSlots = 4, kChunk = 4;
-  uint8_t *slot_in[kSlots] = {nullptr}, *slot_out[kSlots] = {nullptr};
-  cudaStream_t s_h2d = nullptr, s_run = nullptr, s_d2h = nullptr;
-  cudaEvent_t ev_in[kSlots] = {nullptr}, ev_run[kSlots] = {nullptr}, ev_out[kSlots] = {nullptr};
-  bool pipeline_ready = false;
+  HostRing<kSlots> ring;
   int slot_frames = 0;            // frames each slot holds (one kernel launch per slot-full)
   Lanczos2Tables l2_tables;
   Lanczos2State l2;
@@ -529,30 +526,13 @@ int prepare_device (b200_vcs * h)
 
 int ensure_pipeline (b200_vcs * h, int chunk)
 {
-  if (h->pipeline_ready && chunk <= h->slot_frames) return B200_OK;
+  if (chunk <= h->slot_frames) return B200_OK;
   h->in_bytes = b200_video_info_size (&h->plan.in);
   h->out_bytes = b200_video_info_size (&h->plan.frame_out);
-  if (!h->pipeline_ready) {
-    B200_CUDA_TRY (cudaStreamCreateWithFlags (&h->s_h2d, cudaStreamNonBlocking));
-    B200_CUDA_TRY (cudaStreamCreateWithFlags (&h->s_run, cudaStreamNonBlocking));
-    B200_CUDA_TRY (cudaStreamCreateWithFlags (&h->s_d2h, cudaStreamNonBlocking));
-    for (int i = 0; i < b200_vcs::kSlots; i++) {
-      B200_CUDA_TRY (cudaEventCreateWithFlags (&h->ev_in[i], cudaEventDisableTiming));
-      B200_CUDA_TRY (cudaEventCreateWithFlags (&h->ev_run[i], cudaEventDisableTiming));
-      B200_CUDA_TRY (cudaEventCreateWithFlags (&h->ev_out[i], cudaEventDisableTiming));
-    }
-    h->pipeline_ready = true;
-  }
+  B200_CUDA_TRY (h->ring.setup ());
   // (re)size the slots: each holds `chunk` frames, so that one kernel launch and one event triple serve a whole chunk
-  for (int i = 0; i < b200_vcs::kSlots; i++) {
-    B200_CUDA_TRY (cudaFree (h->slot_in[i])); h->slot_in[i] = nullptr;       // cudaFree waits for work still using it
-    B200_CUDA_TRY (cudaFree (h->slot_out[i])); h->slot_out[i] = nullptr;
-  }
   h->slot_frames = 0;
-  for (int i = 0; i < b200_vcs::kSlots; i++) {
-    B200_CUDA_TRY (cudaMalloc ((void **) &h->slot_in[i], h->in_bytes * chunk));
-    B200_CUDA_TRY (cudaMalloc ((void **) &h->slot_out[i], h->out_bytes * chunk));
-  }
+  B200_CUDA_TRY (h->ring.resize (h->in_bytes * chunk, h->out_bytes * chunk));
   h->slot_frames = chunk;
   return B200_OK;
 }
@@ -730,15 +710,7 @@ void b200_vcs_destroy (b200_vcs * h)
     free_planes (&h->planes);
     free_plane_fast (&h->rgb420_scaler);
     cudaFree (h->d_scratch);
-    for (int i = 0; i < b200_vcs::kSlots; i++) {
-      cudaFree (h->slot_in[i]); cudaFree (h->slot_out[i]);
-      if (h->ev_in[i]) cudaEventDestroy (h->ev_in[i]);
-      if (h->ev_run[i]) cudaEventDestroy (h->ev_run[i]);
-      if (h->ev_out[i]) cudaEventDestroy (h->ev_out[i]);
-    }
-    if (h->s_h2d) cudaStreamDestroy (h->s_h2d);
-    if (h->s_run) cudaStreamDestroy (h->s_run);
-    if (h->s_d2h) cudaStreamDestroy (h->s_d2h);
+    h->ring.release ();
   }
   delete h;
 }
@@ -774,33 +746,26 @@ int b200_vcs_convert_host (b200_vcs * h, int n, const void *const *in_host, void
   // Three-stage software pipeline over kSlots device slots of `chunk` frames: the upload of chunk c+1 and the download
   // of chunk c-1 overlap the kernel of chunk c (the copy engines run beside the SMs).  One kernel launch and one event
   // triple per chunk, not per frame; with few frames the chunk shrinks so that all three stages still overlap.
-  const int K = b200_vcs::kSlots;
   // chunks only for long calls: with few frames per call the pipeline's fill and drain would outweigh what chunking saves
   const int chunk = n >= 16 * b200_vcs::kChunk ? b200_vcs::kChunk : (n >= 32 ? 2 : 1);
   int st = ensure_pipeline (h, chunk);
   if (st != B200_OK) return st;
-  int c = 0;
-  for (int i0 = 0; i0 < n; i0 += chunk, c++) {
-    const int s = c % K, m = min (chunk, n - i0);
-    if (c >= K) {
-      B200_CUDA_TRY (cudaStreamWaitEvent (h->s_h2d, h->ev_run[s], 0));   // input slot consumed
-      B200_CUDA_TRY (cudaStreamWaitEvent (h->s_run, h->ev_out[s], 0));   // output slot drained
-    }
+  auto & r = h->ring;
+  for (int i0 = 0; i0 < n; i0 += chunk) {
+    const int m = min (chunk, n - i0);
+    B200_CUDA_TRY (r.take ());
     VcsBatch b;
     for (int j = 0; j < m; j++) {
-      b.in[j] = h->slot_in[s] + (size_t) j * h->in_bytes; b.out[j] = h->slot_out[s] + (size_t) j * h->out_bytes;
-      B200_CUDA_TRY (cudaMemcpyAsync ((void *) b.in[j], in_host[i0 + j], h->in_bytes, cudaMemcpyHostToDevice, h->s_h2d));
+      b.in[j] = r.in () + (size_t) j * h->in_bytes; b.out[j] = r.out () + (size_t) j * h->out_bytes;
+      B200_CUDA_TRY (r.upload ((void *) b.in[j], in_host[i0 + j], h->in_bytes));
     }
-    B200_CUDA_TRY (cudaEventRecord (h->ev_in[s], h->s_h2d));
-    B200_CUDA_TRY (cudaStreamWaitEvent (h->s_run, h->ev_in[s], 0));
-    if ((st = launch_convert (h, m, b, h->s_run)) != B200_OK) return st;
-    B200_CUDA_TRY (cudaEventRecord (h->ev_run[s], h->s_run));
-    B200_CUDA_TRY (cudaStreamWaitEvent (h->s_d2h, h->ev_run[s], 0));
-    for (int j = 0; j < m; j++)
-      B200_CUDA_TRY (cudaMemcpyAsync (out_host[i0 + j], b.out[j], h->out_bytes, cudaMemcpyDeviceToHost, h->s_d2h));
-    B200_CUDA_TRY (cudaEventRecord (h->ev_out[s], h->s_d2h));
+    B200_CUDA_TRY (r.inputs_ready ());
+    if ((st = launch_convert (h, m, b, r.run_stream ())) != B200_OK) return st;
+    B200_CUDA_TRY (r.run_done ());
+    for (int j = 0; j < m; j++) B200_CUDA_TRY (r.download (out_host[i0 + j], b.out[j], h->out_bytes));
+    B200_CUDA_TRY (r.finish ());
   }
-  B200_CUDA_TRY (cudaStreamSynchronize (h->s_d2h));
+  B200_CUDA_TRY (r.drain ());
   return B200_OK;
 }
 
@@ -814,15 +779,14 @@ int b200_vcs_copy_probe (b200_vcs * h, int n, const void *const *in_host, void *
   if (!g.ok) return B200_ERR_CUDA;
   int st = ensure_pipeline (h, max (h->slot_frames, 1));
   if (st != B200_OK) return st;
-  const int K = b200_vcs::kSlots, chunk = h->slot_frames;
+  const int chunk = h->slot_frames;
   for (int i = 0; i < n; i++) {
-    const int s = (i / chunk) % K, j = i % chunk;
+    const int s = (i / chunk) % b200_vcs::kSlots, j = i % chunk;
     if (!in_host[i] || !out_host[i]) return B200_ERR_INVALID_ARG;
-    B200_CUDA_TRY (cudaMemcpyAsync (h->slot_in[s] + (size_t) j * h->in_bytes, in_host[i], h->in_bytes, cudaMemcpyHostToDevice, h->s_h2d));
-    B200_CUDA_TRY (cudaMemcpyAsync (out_host[i], h->slot_out[s] + (size_t) j * h->out_bytes, h->out_bytes, cudaMemcpyDeviceToHost, h->s_d2h));
+    B200_CUDA_TRY (h->ring.upload (h->ring.in (s) + (size_t) j * h->in_bytes, in_host[i], h->in_bytes));
+    B200_CUDA_TRY (h->ring.download (out_host[i], h->ring.out (s) + (size_t) j * h->out_bytes, h->out_bytes));
   }
-  B200_CUDA_TRY (cudaStreamSynchronize (h->s_h2d));
-  B200_CUDA_TRY (cudaStreamSynchronize (h->s_d2h));
+  B200_CUDA_TRY (h->ring.drain (true));                           // the copies of both directions are unordered
   return B200_OK;
 }
 

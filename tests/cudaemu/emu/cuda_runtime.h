@@ -132,20 +132,32 @@ inline unsigned __vavgu4 (unsigned a, unsigned b)
 
 // ---- runtime API subset -----------------------------------------------------------------------------------------------
 typedef int cudaError_t;
-enum { cudaSuccess = 0, cudaErrorMemoryAllocation = 2, cudaErrorNoDevice = 100, cudaErrorInsufficientDriver = 35 };
+enum { cudaSuccess = 0, cudaErrorMemoryAllocation = 2, cudaErrorNoDevice = 100, cudaErrorInsufficientDriver = 35,
+       cudaErrorUnknown = 999 };
 typedef void *cudaStream_t;
 typedef void *cudaEvent_t;
 enum cudaMemcpyKind { cudaMemcpyHostToDevice = 1, cudaMemcpyDeviceToHost = 2, cudaMemcpyDeviceToDevice = 3 };
 enum { cudaStreamNonBlocking = 1, cudaEventDisableTiming = 2, cudaHostAllocPortable = 1, cudaHostRegisterPortable = 1 };
 enum { cudaFuncAttributeMaxDynamicSharedMemorySize = 8, cudaDevAttrMultiProcessorCount = 16, cudaDevAttrMaxSharedMemoryPerBlockOptin = 97 };
 
-inline cudaError_t cudaMalloc (void **p, size_t n) { *p = malloc (n ? n : 1); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
-inline cudaError_t cudaFree (void *p) { free (p); return cudaSuccess; }
+// emu_runtime.cpp: device allocations, copies and the stream / event calls.  Work runs at once on the calling thread;
+// at record level 3 each call is logged (b200emu_launch_log).  Streams and events are distinct non-null handles.
+cudaError_t cudaMalloc (void **p, size_t n);
+cudaError_t cudaFree (void *p);
+cudaError_t cudaMemsetAsync (void *d, int v, size_t n, cudaStream_t s);
+cudaError_t cudaMemcpyAsync (void *d, const void *s, size_t n, cudaMemcpyKind k, cudaStream_t st);
+cudaError_t cudaDeviceSynchronize ();
+cudaError_t cudaStreamCreateWithFlags (cudaStream_t *s, unsigned flags);
+cudaError_t cudaStreamDestroy (cudaStream_t s);
+cudaError_t cudaStreamSynchronize (cudaStream_t s);
+cudaError_t cudaStreamWaitEvent (cudaStream_t s, cudaEvent_t e, unsigned flags);
+cudaError_t cudaEventCreateWithFlags (cudaEvent_t *e, unsigned flags);
+cudaError_t cudaEventDestroy (cudaEvent_t e);
+cudaError_t cudaEventRecord (cudaEvent_t e, cudaStream_t s);
+cudaError_t cudaEventSynchronize (cudaEvent_t e);
+
 inline cudaError_t cudaMemcpy (void *d, const void *s, size_t n, cudaMemcpyKind) { memcpy (d, s, n); return cudaSuccess; }
 inline cudaError_t cudaMemset (void *d, int v, size_t n) { memset (d, v, n); return cudaSuccess; }
-inline cudaError_t cudaMemsetAsync (void *d, int v, size_t n, cudaStream_t) { memset (d, v, n); return cudaSuccess; }
-inline cudaError_t cudaDeviceSynchronize () { return cudaSuccess; }
-inline cudaError_t cudaMemcpyAsync (void *d, const void *s, size_t n, cudaMemcpyKind, cudaStream_t) { memcpy (d, s, n); return cudaSuccess; }
 inline cudaError_t cudaGetLastError () { return cudaSuccess; }
 inline const char *cudaGetErrorName (cudaError_t) { return "emu"; }
 inline const char *cudaGetErrorString (cudaError_t) { return "emu"; }
@@ -153,14 +165,6 @@ inline cudaError_t cudaGetDevice (int *d) { *d = 0; return cudaSuccess; }
 inline cudaError_t cudaSetDevice (int) { return cudaSuccess; }
 inline cudaError_t cudaGetDeviceCount (int *n) { *n = 1; return cudaSuccess; }
 inline cudaError_t cudaDeviceGetAttribute (int *v, int a, int) { *v = a == cudaDevAttrMaxSharedMemoryPerBlockOptin ? 232448 : 148; return cudaSuccess; }
-inline cudaError_t cudaStreamCreateWithFlags (cudaStream_t *s, unsigned) { *s = nullptr; return cudaSuccess; }
-inline cudaError_t cudaStreamDestroy (cudaStream_t) { return cudaSuccess; }
-inline cudaError_t cudaStreamSynchronize (cudaStream_t) { return cudaSuccess; }
-inline cudaError_t cudaStreamWaitEvent (cudaStream_t, cudaEvent_t, unsigned) { return cudaSuccess; }
-inline cudaError_t cudaEventCreateWithFlags (cudaEvent_t *e, unsigned) { *e = nullptr; return cudaSuccess; }
-inline cudaError_t cudaEventDestroy (cudaEvent_t) { return cudaSuccess; }
-inline cudaError_t cudaEventRecord (cudaEvent_t, cudaStream_t) { return cudaSuccess; }
-inline cudaError_t cudaEventSynchronize (cudaEvent_t) { return cudaSuccess; }
 inline cudaError_t cudaHostAlloc (void **p, size_t n, unsigned) { *p = malloc (n); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
 inline cudaError_t cudaFreeHost (void *p) { free (p); return cudaSuccess; }
 inline cudaError_t cudaHostRegister (void *, size_t, unsigned) { return cudaSuccess; }

@@ -9,6 +9,7 @@
 #include <dlfcn.h>
 
 #include <condition_variable>
+#include <map>
 #include <mutex>
 #include <string>
 
@@ -189,15 +190,144 @@ void launch (dim3 grid, dim3 block, size_t smem_bytes, const std::function<void 
   free (smem);
 }
 
+// ---- allocations, copies, streams and events ------------------------------------------------------------------------
+// Handles and allocations are named by creation order since the last log clear (s0, e0, a0, ...; "?" for one created
+// before it), so a level-3 log holds no addresses.
+static std::map<uintptr_t, std::pair<size_t, std::string>> g_allocs;    // base -> (bytes, name)
+static std::map<void *, std::string> g_handles;                        // stream / event -> name
+static int g_n_alloc = 0, g_n_stream = 0, g_n_event = 0;
+static int g_fail_create = 0;                  // > 0: the n-th stream or event creation from now fails
+
+static void note (const std::string & line)
+{
+  if (g_record_only >= 3) g_log += line + '\n';
+}
+
+static std::string handle_name (void *h)
+{
+  if (!h) return "0";                          // the legacy default stream
+  auto it = g_handles.find (h);
+  return it == g_handles.end () ? "?" : it->second;
+}
+
+// "a<k>+<offset>" for a pointer into a device allocation, "host" for any other
+static std::string where (const void *p)
+{
+  const uintptr_t a = (uintptr_t) p;
+  auto it = g_allocs.upper_bound (a);
+  if (it == g_allocs.begin ()) return "host";
+  --it;
+  if (a >= it->first + std::max<size_t> (it->second.first, 1)) return "host";
+  return it->second.second + "+" + std::to_string (a - it->first);
+}
+
+static bool create_fails ()
+{
+  return g_fail_create > 0 && --g_fail_create == 0;
+}
+
+static void forget_names ()
+{
+  for (auto & a : g_allocs) a.second.second = "?";
+  for (auto & h : g_handles) h.second = "?";
+  g_n_alloc = g_n_stream = g_n_event = 0;
+}
+
 }  // namespace b200emu
+
+using namespace b200emu;
+
+cudaError_t cudaMalloc (void **p, size_t n)
+{
+  *p = malloc (n ? n : 1);
+  if (!*p) return cudaErrorMemoryAllocation;
+  const std::string name = "a" + std::to_string (g_n_alloc++);
+  g_allocs[(uintptr_t) *p] = {n, name};
+  note ("cudaMalloc " + name + " bytes=" + std::to_string (n));
+  return cudaSuccess;
+}
+
+cudaError_t cudaFree (void *p)
+{
+  if (!p) { note ("cudaFree null"); return cudaSuccess; }
+  auto it = g_allocs.find ((uintptr_t) p);
+  note ("cudaFree " + (it == g_allocs.end () ? std::string ("host") : it->second.second));
+  if (it != g_allocs.end ()) g_allocs.erase (it);
+  free (p);
+  return cudaSuccess;
+}
+
+cudaError_t cudaMemsetAsync (void *d, int v, size_t n, cudaStream_t s)
+{
+  note ("cudaMemsetAsync " + where (d) + " value=" + std::to_string (v) + " bytes=" + std::to_string (n) + " stream=" + handle_name (s));
+  memset (d, v, n);
+  return cudaSuccess;
+}
+
+cudaError_t cudaMemcpyAsync (void *d, const void *s, size_t n, cudaMemcpyKind k, cudaStream_t st)
+{
+  const char *dir = k == cudaMemcpyHostToDevice ? "H2D" : (k == cudaMemcpyDeviceToHost ? "D2H" : "D2D");
+  std::string line = std::string ("cudaMemcpyAsync ") + dir + " bytes=" + std::to_string (n) + " stream=" + handle_name (st);
+  if (k != cudaMemcpyHostToDevice) line += " src=" + where (s);
+  if (k != cudaMemcpyDeviceToHost) line += " dst=" + where (d);
+  note (line);
+  memcpy (d, s, n);
+  return cudaSuccess;
+}
+
+cudaError_t cudaDeviceSynchronize () { note ("cudaDeviceSynchronize"); return cudaSuccess; }
+
+cudaError_t cudaStreamCreateWithFlags (cudaStream_t *s, unsigned)
+{
+  if (create_fails ()) { note ("cudaStreamCreate failed"); return cudaErrorUnknown; }
+  *s = new char;
+  g_handles[*s] = "s" + std::to_string (g_n_stream++);
+  note ("cudaStreamCreate " + g_handles[*s]);
+  return cudaSuccess;
+}
+
+cudaError_t cudaEventCreateWithFlags (cudaEvent_t *e, unsigned)
+{
+  if (create_fails ()) { note ("cudaEventCreate failed"); return cudaErrorUnknown; }
+  *e = new char;
+  g_handles[*e] = "e" + std::to_string (g_n_event++);
+  note ("cudaEventCreate " + g_handles[*e]);
+  return cudaSuccess;
+}
+
+static cudaError_t destroy_handle (const char *what, void *h)
+{
+  note (std::string (what) + " " + handle_name (h));
+  g_handles.erase (h);
+  delete (char *) h;
+  return cudaSuccess;
+}
+
+cudaError_t cudaStreamDestroy (cudaStream_t s) { return destroy_handle ("cudaStreamDestroy", s); }
+cudaError_t cudaEventDestroy (cudaEvent_t e) { return destroy_handle ("cudaEventDestroy", e); }
+cudaError_t cudaStreamSynchronize (cudaStream_t s) { note ("cudaStreamSynchronize " + handle_name (s)); return cudaSuccess; }
+cudaError_t cudaEventSynchronize (cudaEvent_t e) { note ("cudaEventSynchronize " + handle_name (e)); return cudaSuccess; }
+cudaError_t cudaEventRecord (cudaEvent_t e, cudaStream_t s)
+{
+  note ("cudaEventRecord " + handle_name (e) + " stream=" + handle_name (s));
+  return cudaSuccess;
+}
+cudaError_t cudaStreamWaitEvent (cudaStream_t s, cudaEvent_t e, unsigned)
+{
+  note ("cudaStreamWaitEvent stream=" + handle_name (s) + " " + handle_name (e));
+  return cudaSuccess;
+}
 
 extern "C" {
 
 // the kernels launched since the last clear, one name per line (valid until the next launch or clear)
 const char *b200emu_launch_log () { return b200emu::g_log.c_str (); }
-void b200emu_clear_launch_log () { b200emu::g_log.clear (); }
+void b200emu_clear_launch_log () { b200emu::g_log.clear (); b200emu::forget_names (); }
 // 1: launches are logged by kernel and no block runs (route tests); 2: the same, each line followed by
-// " grid=x,y,z block=x,y,z smem=bytes"; 0 (the default): launches run and are not logged
+// " grid=x,y,z block=x,y,z smem=bytes"; 3: level 2 and, in between, the allocations, copies, memsets and stream / event
+// calls; 0 (the default): launches run and nothing is logged
 void b200emu_set_record_only (int level) { b200emu::g_record_only = level; }
+// test hook: the n-th stream or event creation from now fails with an error (0: none fails)
+void b200emu_fail_create (int n) { b200emu::g_fail_create = n; }
 
 }
