@@ -398,6 +398,78 @@ __device__ __forceinline__ void ars_position (const ArsLaunch & L, long long o, 
   phase = (int) (t % L.out_step);
 }
 
+// the samples of stream frame f: a row of the retained history, a row of the caller's input, or nullptr (silence)
+template <typename T>
+__device__ __forceinline__ const T *ars_frame_row (const ArsLaunch & L, long long f)
+{
+  const T *src = nullptr;
+  if (f < L.hist_frames) src = (const T *) L.hist + f * L.channels;
+  else if (f < L.avail && L.in) src = (const T *) L.in + (f - L.hist_frames) * L.channels;
+  return src;
+}
+
+// (l0 + l2) + (l1 + l3): the final reduction of the four partial sums, audio-resampler-x86-sse.c:43-45
+__device__ __forceinline__ float ars_lane_sum (const float l[4])
+{
+  return __fadd_rn (__fadd_rn (l[0], l[2]), __fadd_rn (l[1], l[3]));
+}
+
+// The F32 inner products of one group of RQ consecutive outputs for CPT adjacent channels over a staged [frame][CB]
+// window: xp = the thread's first channel at the group's first (chunk-aligned) frame, tp = the group's chunk-major taps
+// (RQ float4 per chunk), nch chunks.  Four partial sums per (channel, output) by tap index mod 4, separate multiply and
+// add (no FMA); ars_lane_sum reduces them.
+template <int CPT, int CB>
+__device__ __forceinline__ void ars_group_f32 (const float *xp, const float4 *tp, int nch, float (&acc)[CPT][ARS_RQ][4])
+{
+  constexpr int RQ = ARS_RQ;
+#pragma unroll
+  for (int u = 0; u < CPT; u++)
+#pragma unroll
+    for (int r = 0; r < RQ; r++)
+#pragma unroll
+      for (int k = 0; k < 4; k++) acc[u][r][k] = 0.f;
+#pragma unroll 2
+  for (int ch = 0; ch < nch; ch++, xp += 4 * CB, tp += RQ) {
+    float x[CPT][4];
+    if (CPT == 4) {
+#pragma unroll
+      for (int k = 0; k < 4; k++) {
+        const float4 v = *(const float4 *) (xp + k * CB);
+        x[0][k] = v.x; x[1 % CPT][k] = v.y; x[2 % CPT][k] = v.z; x[3 % CPT][k] = v.w;
+      }
+    } else if (CPT == 2) {
+#pragma unroll
+      for (int k = 0; k < 4; k++) {
+        const float2 v = *(const float2 *) (xp + k * CB);
+        x[0][k] = v.x; x[CPT - 1][k] = v.y;
+      }
+    } else {
+#pragma unroll
+      for (int k = 0; k < 4; k++) x[0][k] = xp[k * CB];
+    }
+#pragma unroll
+    for (int r = 0; r < RQ; r++) {
+      const float4 t = tp[r];
+#pragma unroll
+      for (int u = 0; u < CPT; u++) {
+        acc[u][r][0] = __fadd_rn (acc[u][r][0], __fmul_rn (x[u][0], t.x));
+        acc[u][r][1] = __fadd_rn (acc[u][r][1], __fmul_rn (x[u][1], t.y));
+        acc[u][r][2] = __fadd_rn (acc[u][r][2], __fmul_rn (x[u][2], t.z));
+        acc[u][r][3] = __fadd_rn (acc[u][r][3], __fmul_rn (x[u][3], t.w));
+      }
+    }
+  }
+}
+
+// the integer inner products' rounding: the S16 sum (wrapped to 32 bits) + 2^14, >> 15, saturated
+// (audio-resampler-x86-sse2.c:48-54); the S32 sum (wrapped to 64 bits) + 2^30, >> 31, saturated
+__device__ __forceinline__ int ars_round_s16 (unsigned sum) { return min (max ((int) (sum + (1u << 14)) >> 15, -32768), 32767); }
+__device__ __forceinline__ int ars_round_s32 (unsigned long long sum)
+{
+  const long long v = ((long long) sum + (1 << 30)) >> 31;
+  return (int) (v < -2147483648LL ? -2147483648LL : (v > 2147483647LL ? 2147483647LL : v));
+}
+
 __global__ void __launch_bounds__ (ARS_THREADS)
 ars_full_kernel (const ArsLaunch L)
 {
@@ -442,6 +514,7 @@ ars_full_kernel (const ArsLaunch L)
       float x[4];
 #pragma unroll
       for (int j = 0; j < 4; j++) {
+        // two loads rather than ars_frame_row's pointer: selecting the row first costs this kernel two registers
         const long long f = s4 + j;
         float v = 0.f;
         if (f < L.hist_frames) v = __ldg (L.hist + f * L.channels + cc);
@@ -469,11 +542,7 @@ ars_full_kernel (const ArsLaunch L)
     }
 #pragma unroll
     for (int r = 0; r < ARS_RQ; r++) {
-      if (q + r < n_out && c_ok) {
-        // (l0 + l2) + (l1 + l3), audio-resampler-x86-sse.c:43-45
-        const float v = __fadd_rn (__fadd_rn (acc[r][0], acc[r][2]), __fadd_rn (acc[r][1], acc[r][3]));
-        L.out[(size_t) (o0 + q + r) * L.channels + c] = v;
-      }
+      if (q + r < n_out && c_ok) L.out[(size_t) (o0 + q + r) * L.channels + c] = ars_lane_sum (acc[r]);
     }
   }
 }
@@ -511,45 +580,26 @@ static size_t ars_tile_smem (const ArsTile & t, int no, int cb, int sample_bytes
   return (size_t) (no / ARS_RQ) * t.nch * ARS_RQ * 4 * sizeof (float) + (size_t) t.win * cb * sample_bytes;
 }
 
-// host side of the layout above; nch from ars_tile_geometry
-static void ars_build_qtab (const ArsPlan & p, int nch, std::vector<float> * out)
+// host side of the layout above; phases = [phase][n_taps] taps of type Tap, stored as Wide (4 bytes: F32 taps as they
+// are, the S16 resampler's int16 taps widened to int32); nch from ars_tile_geometry
+template <typename Tap, typename Wide>
+static void ars_build_qtab (const ArsPlan & p, const Tap *phases, int nch, std::vector<float> * out)
 {
+  static_assert (sizeof (Wide) == sizeof (float), "the table is uploaded as floats");
   const int RQ = 4;
   out->assign ((size_t) 4 * p.out_step * nch * RQ * 4, 0.f);
+  Wide *o = (Wide *) out->data ();
   for (int a = 0; a < 4; a++)
     for (int ph = 0; ph < p.out_step; ph++)
       for (int r = 0; r < RQ; r++) {
         const long long t = (long long) ph + (long long) r * p.samp_frac;
         const int delta = (int) ((long long) r * p.samp_inc + t / p.out_step), phase = (int) (t % p.out_step);
-        const float *src = &p.phases[(size_t) phase * p.n_taps];
+        const Tap *src = phases + (size_t) phase * p.n_taps;
         for (int chunk = 0; chunk < nch; chunk++) {
-          float *dst = &(*out)[((((size_t) a * p.out_step + ph) * nch + chunk) * RQ + r) * 4];
+          Wide *dst = o + ((((size_t) a * p.out_step + ph) * nch + chunk) * RQ + r) * 4;
           for (int k = 0; k < 4; k++) {
             const int tap = 4 * chunk + k - (a + delta);
-            dst[k] = (tap >= 0 && tap < p.n_taps) ? src[tap] : 0.f;
-          }
-        }
-      }
-}
-
-// the same layout with the S16 resampler's integer taps widened to 32 bits (phases_x holds them as int16, [phase][n_taps])
-static void ars_build_qtab_s16 (const ArsPlan & p, int nch, std::vector<float> * out)
-{
-  const int RQ = 4;
-  out->assign ((size_t) 4 * p.out_step * nch * RQ * 4, 0.f);
-  const int16_t *phases = (const int16_t *) p.phases_x.data ();
-  int32_t *o = (int32_t *) out->data ();
-  for (int a = 0; a < 4; a++)
-    for (int ph = 0; ph < p.out_step; ph++)
-      for (int r = 0; r < RQ; r++) {
-        const long long t = (long long) ph + (long long) r * p.samp_frac;
-        const int delta = (int) ((long long) r * p.samp_inc + t / p.out_step), phase = (int) (t % p.out_step);
-        const int16_t *src = phases + (size_t) phase * p.n_taps;
-        for (int chunk = 0; chunk < nch; chunk++) {
-          int32_t *dst = o + ((((size_t) a * p.out_step + ph) * nch + chunk) * RQ + r) * 4;
-          for (int k = 0; k < 4; k++) {
-            const int tap = 4 * chunk + k - (a + delta);
-            dst[k] = (tap >= 0 && tap < p.n_taps) ? (int32_t) src[tap] : 0;
+            dst[k] = (tap >= 0 && tap < p.n_taps) ? (Wide) src[tap] : (Wide) 0;
           }
         }
       }
@@ -586,10 +636,7 @@ ars_tile_kernel (const ArsLaunch L, const ArsTile Tl)
   const bool vec = CB == 128 && (L.channels & 3) == 0 && c_base + CB <= L.channels &&
       ((((uintptr_t) L.hist) | ((uintptr_t) L.in)) & 15) == 0;
   for (int fr = warp; fr < Tl.win; fr += ARS_THREADS / 32) {
-    const long long f = f0 + fr;
-    const float *src = nullptr;
-    if (f < L.hist_frames) src = L.hist + f * L.channels;
-    else if (f < L.avail && L.in) src = L.in + (f - L.hist_frames) * L.channels;
+    const float *src = ars_frame_row<float> (L, f0 + fr);
     if (vec) {
       *(float4 *) (xin + fr * CB + 4 * lane) = src ? __ldg ((const float4 *) (src + c_base) + lane) : make_float4 (0.f, 0.f, 0.f, 0.f);
     } else {
@@ -617,68 +664,24 @@ ars_tile_kernel (const ArsLaunch L, const ArsTile Tl)
   constexpr int NOG = (ARS_THREADS / 32) / WCN;
   const int cl = (cg * 32 + lane) * CPT, c = c_base + cl;
   for (int q = og; q < nq; q += NOG) {
-    float acc[CPT][RQ][4];
-#pragma unroll
-    for (int u = 0; u < CPT; u++)
-#pragma unroll
-      for (int r = 0; r < RQ; r++)
-#pragma unroll
-        for (int k = 0; k < 4; k++) acc[u][r][k] = 0.f;
     const int s_min = s_rel[q * RQ] & ~3;
     const int s_max = (s_rel[min (q * RQ + RQ - 1, n_out - 1)] + L.n_taps + 3) & ~3;
     const int nch = (s_max - s_min) >> 2;
     const float *xp = xin + s_min * CB + cl;
     const float4 *tp = qt + (size_t) q * Tl.nch * RQ;
-#pragma unroll 2
-    for (int ch = 0; ch < nch; ch++, xp += 4 * CB, tp += RQ) {
-      float x[CPT][4];
-      if (CPT == 4) {
-#pragma unroll
-        for (int k = 0; k < 4; k++) {
-          const float4 v = *(const float4 *) (xp + k * CB);
-          x[0][k] = v.x; x[1 % CPT][k] = v.y; x[2 % CPT][k] = v.z; x[3 % CPT][k] = v.w;
-        }
-      } else if (CPT == 2) {
-#pragma unroll
-        for (int k = 0; k < 4; k++) {
-          const float2 v = *(const float2 *) (xp + k * CB);
-          x[0][k] = v.x; x[CPT - 1][k] = v.y;
-        }
-      } else {
-#pragma unroll
-        for (int k = 0; k < 4; k++) x[0][k] = xp[k * CB];
-      }
-#pragma unroll
-      for (int r = 0; r < RQ; r++) {
-        const float4 t = tp[r];
-#pragma unroll
-        for (int u = 0; u < CPT; u++) {
-          acc[u][r][0] = __fadd_rn (acc[u][r][0], __fmul_rn (x[u][0], t.x));
-          acc[u][r][1] = __fadd_rn (acc[u][r][1], __fmul_rn (x[u][1], t.y));
-          acc[u][r][2] = __fadd_rn (acc[u][r][2], __fmul_rn (x[u][2], t.z));
-          acc[u][r][3] = __fadd_rn (acc[u][r][3], __fmul_rn (x[u][3], t.w));
-        }
-      }
-    }
+    float acc[CPT][RQ][4];
+    ars_group_f32<CPT, CB> (xp, tp, nch, acc);
 #pragma unroll
     for (int r = 0; r < RQ; r++) {
 #pragma unroll
       for (int u = 0; u < CPT; u++) {
-        if (q * RQ + r < n_out && c + u < L.channels) {
-          const float v = __fadd_rn (__fadd_rn (acc[u][r][0], acc[u][r][2]), __fadd_rn (acc[u][r][1], acc[u][r][3]));
-          L.out[(size_t) (o0 + q * RQ + r) * L.channels + c + u] = v;
-        }
+        if (q * RQ + r < n_out && c + u < L.channels)
+          L.out[(size_t) (o0 + q * RQ + r) * L.channels + c + u] = ars_lane_sum (acc[u][r]);
       }
     }
   }
 }
 
-__device__ __forceinline__ int sat_s16 (int v) { return min (max (v, -32768), 32767); }
-__device__ __forceinline__ long long sat_s32 (long long v) { return v < -2147483648LL ? -2147483648LL : (v > 2147483647LL ? 2147483647LL : v); }
-
-// S16 samples through the same tiling: the window is staged widened to 32 bits, taps likewise; the sums are
-// integers (wrapping 32 bit like the SSE2 pmaddwd path), so no lane structure has to be kept —
-// inner_product_gint16_full_1_sse2 (audio-resampler-x86-sse2.c:29-56): sum, + 2^14, >> 15, saturate.
 // ---- ars_pipe_kernel: the tile kernel as a persistent, double-buffered pipeline ------------------------------------------
 // In ars_tile_kernel on the C5 shape the prologue (window and tap rows travelling from L2 to shared memory) stalls far more
 // than its share of the instructions - two CTAs per SM cannot hide it.
@@ -688,6 +691,88 @@ __device__ __forceinline__ long long sat_s32 (long long v) { return v < -2147483
 // one LDS.128 of samples and one broadcast LDS.128 of taps feed 32 FMUL + 32 FADD.  Arithmetic and its order are those of
 // ars_tile_kernel (four partial sums by tap index mod 4, (l0 + l2) + (l1 + l3), no FMA): bit-identical output.
 constexpr int ARS_PIPE_THREADS = 512, ARS_PIPE_NO = 64, ARS_PIPE_CB = 128;
+
+// sign-extending byte permute: the 16-bit sample in the low (0x9910) or high (0xbb32) half of a word as an int
+__device__ __forceinline__ int prmt_s16 (unsigned v, unsigned sel)
+{
+#ifdef B200_CUDA_EMU
+  return sel == 0x9910u ? (int) (short) (v & 0xffffu) : (int) (short) (v >> 16);
+#else
+  int d;
+  asm ("prmt.b32 %0, %1, 0, %2;" : "=r" (d) : "r" (v), "r" (sel));
+  return d;
+#endif
+}
+
+// What the pipelines do per sample format: the staged Sample type (which sets the stage layout and the copy sizes), the
+// Tap vector of one chunk of the tap rows, and group (): a warp's 4-output group for its lane's 4 adjacent channels c ..
+// c + 3 - xp, tp and nch as for ars_group_f32; outputs o0 + q0 .. o0 + q0 + 3 of the stream, those below the tile's n_out
+// stored.
+struct ArsPipeF32 {
+  typedef float Sample;
+  typedef float4 Tap;
+  static __device__ __forceinline__ void group (const ArsLaunch & L, const float *xp, const float4 *tp, int nch, long long o0, int q0, int c, int n_out)
+  {
+    float acc[4][ARS_RQ][4];
+    ars_group_f32<4, ARS_PIPE_CB> (xp, tp, nch, acc);
+    float *op = L.out + (size_t) (o0 + q0) * L.channels + c;
+#pragma unroll
+    for (int r = 0; r < ARS_RQ; r++) {
+      if (q0 + r < n_out) {
+        float4 o;
+        o.x = ars_lane_sum (acc[0][r]); o.y = ars_lane_sum (acc[1][r]); o.z = ars_lane_sum (acc[2][r]); o.w = ars_lane_sum (acc[3][r]);
+        *(float4 *) (op + (size_t) r * L.channels) = o;
+      }
+    }
+  }
+};
+
+// The window travels as raw 16-bit samples, the tap rows as 32-bit ints in the F32 chunk-major layout: per frame position
+// one LDS.64 of samples (4 sign-extending PRMT) and per output one broadcast LDS.128 of taps feed 16 IMAD.  Integer sums
+// wrap in 32 bits like the SSE2 pmaddwd path (inner_product_gint16_full_1_sse2, audio-resampler-x86-sse2.c:29-56): no lane
+// structure to keep, one accumulator per (channel, output).
+struct ArsPipeS16 {
+  typedef short Sample;
+  typedef int4 Tap;
+  static __device__ __forceinline__ void group (const ArsLaunch & L, const short *xp, const int4 *tp, int nch, long long o0, int q0, int c, int n_out)
+  {
+    constexpr int RQ = ARS_RQ, CB = ARS_PIPE_CB;
+    unsigned acc[4][RQ];
+#pragma unroll
+    for (int u = 0; u < 4; u++)
+#pragma unroll
+      for (int r = 0; r < RQ; r++) acc[u][r] = 0u;
+#pragma unroll 2
+    for (int ch = 0; ch < nch; ch++, xp += 4 * CB, tp += RQ) {
+      int x[4][4];
+#pragma unroll
+      for (int kk = 0; kk < 4; kk++) {
+        const uint2 v = *(const uint2 *) (xp + kk * CB);           // 4 adjacent channels of one frame, 16 bits each
+        x[0][kk] = prmt_s16 (v.x, 0x9910u); x[1][kk] = prmt_s16 (v.x, 0xbb32u);
+        x[2][kk] = prmt_s16 (v.y, 0x9910u); x[3][kk] = prmt_s16 (v.y, 0xbb32u);
+      }
+#pragma unroll
+      for (int r = 0; r < RQ; r++) {
+        const int4 tq = tp[r];
+#pragma unroll
+        for (int u = 0; u < 4; u++)
+          acc[u][r] += (unsigned) (x[u][0] * tq.x) + (unsigned) (x[u][1] * tq.y) + (unsigned) (x[u][2] * tq.z) + (unsigned) (x[u][3] * tq.w);
+      }
+    }
+    short *op = (short *) L.out + (size_t) (o0 + q0) * L.channels + c;
+#pragma unroll
+    for (int r = 0; r < RQ; r++) {
+      if (q0 + r < n_out) {
+        const int v0 = ars_round_s16 (acc[0][r]), v1 = ars_round_s16 (acc[1][r]);
+        const int v2 = ars_round_s16 (acc[2][r]), v3 = ars_round_s16 (acc[3][r]);
+        uint2 o;
+        o.x = ((unsigned) v0 & 0xffffu) | ((unsigned) v1 << 16);
+        o.y = ((unsigned) v2 & 0xffffu) | ((unsigned) v3 << 16);
+        *(uint2 *) (op + (size_t) r * L.channels) = o;
+      }
+    }
+  }
+};
 
 __device__ __forceinline__ void ars_cp16 (void *dst_smem, const void *src, bool real)
 {
@@ -734,10 +819,7 @@ ars_pipe_kernel_v1 (const ArsLaunch L, const ArsTile Tl, int n_fb, int n_cb)
     const long long f0 = s_f0[ps];
     const int c_base = (t % n_cb) * CB;
     for (int fr = warp; fr < Tl.win; fr += ARS_PIPE_THREADS / 32) {
-      const long long f = f0 + fr;
-      const float *src = nullptr;
-      if (f < L.hist_frames) src = L.hist + f * L.channels;
-      else if (f < L.avail && L.in) src = L.in + (f - L.hist_frames) * L.channels;
+      const float *src = ars_frame_row<float> (L, f0 + fr);
       ars_cp16 (xin + fr * CB + 4 * lane, src ? (const void *) (src + c_base + 4 * lane) : (const void *) Tl.qtab, src != nullptr);
     }
     const int e = threadIdx.x & 127, qq = threadIdx.x >> 7;
@@ -771,46 +853,15 @@ ars_pipe_kernel_v1 (const ArsLaunch L, const ArsTile Tl, int n_fb, int n_cb)
     const int nq = (n_out + RQ - 1) / RQ;
     const int c = (t % n_cb) * CB + 4 * lane;
     for (int q = warp; q < nq; q += ARS_PIPE_THREADS / 32) {
-      float acc[4][RQ][4];
-#pragma unroll
-      for (int u = 0; u < 4; u++)
-#pragma unroll
-        for (int r = 0; r < RQ; r++)
-#pragma unroll
-          for (int k = 0; k < 4; k++) acc[u][r][k] = 0.f;
       const int s_min = s_rel[ps][q * RQ] & ~3;
       const int s_max = (s_rel[ps][min (q * RQ + RQ - 1, n_out - 1)] + L.n_taps + 3) & ~3;
-      const int nch = (s_max - s_min) >> 2;
-      const float *xp = xin + s_min * CB + 4 * lane;
-      const float4 *tp = qt + (size_t) q * row;
-#pragma unroll 2
-      for (int ch = 0; ch < nch; ch++, xp += 4 * CB, tp += RQ) {
-        float x[4][4];
-#pragma unroll
-        for (int k = 0; k < 4; k++) {
-          const float4 v = *(const float4 *) (xp + k * CB);
-          x[0][k] = v.x; x[1][k] = v.y; x[2][k] = v.z; x[3][k] = v.w;
-        }
-#pragma unroll
-        for (int r = 0; r < RQ; r++) {
-          const float4 tq = tp[r];
-#pragma unroll
-          for (int u = 0; u < 4; u++) {
-            acc[u][r][0] = __fadd_rn (acc[u][r][0], __fmul_rn (x[u][0], tq.x));
-            acc[u][r][1] = __fadd_rn (acc[u][r][1], __fmul_rn (x[u][1], tq.y));
-            acc[u][r][2] = __fadd_rn (acc[u][r][2], __fmul_rn (x[u][2], tq.z));
-            acc[u][r][3] = __fadd_rn (acc[u][r][3], __fmul_rn (x[u][3], tq.w));
-          }
-        }
-      }
+      float acc[4][RQ][4];
+      ars_group_f32<4, CB> (xin + s_min * CB + 4 * lane, qt + (size_t) q * row, (s_max - s_min) >> 2, acc);
 #pragma unroll
       for (int r = 0; r < RQ; r++) {
         if (q * RQ + r < n_out) {
           float4 o;
-          o.x = __fadd_rn (__fadd_rn (acc[0][r][0], acc[0][r][2]), __fadd_rn (acc[0][r][1], acc[0][r][3]));
-          o.y = __fadd_rn (__fadd_rn (acc[1][r][0], acc[1][r][2]), __fadd_rn (acc[1][r][1], acc[1][r][3]));
-          o.z = __fadd_rn (__fadd_rn (acc[2][r][0], acc[2][r][2]), __fadd_rn (acc[2][r][1], acc[2][r][3]));
-          o.w = __fadd_rn (__fadd_rn (acc[3][r][0], acc[3][r][2]), __fadd_rn (acc[3][r][1], acc[3][r][3]));
+          o.x = ars_lane_sum (acc[0][r]); o.y = ars_lane_sum (acc[1][r]); o.z = ars_lane_sum (acc[2][r]); o.w = ars_lane_sum (acc[3][r]);
           *(float4 *) (L.out + (size_t) (o0 + q * RQ + r) * L.channels + c) = o;
         }
       }
@@ -918,314 +969,130 @@ __device__ __forceinline__ void ars_warp_sync ()
 #endif
 }
 
+// The pipeline of both sample formats; S (ArsPipeF32, ArsPipeS16) gives the staged sample type and the arithmetic.  A
+// stage = the tap rows (NQ groups x nch chunks of 4-tap vectors) + the window (win frames x CB samples).
+template <class S>
+__device__ __forceinline__ void ars_pipe_body (const ArsLaunch & L, const ArsTile & Tl, int n_fb, int n_cb, const ArsTensorMap *tm_in, int use_tm)
+{
+  typedef typename S::Sample Sample;
+  extern __shared__ __align__ (128) float smp[];
+  constexpr int RQ = ARS_RQ, NO = ARS_PIPE_NO, CB = ARS_PIPE_CB, NQ = NO / RQ, NW = ARS_PIPE_THREADS / 32;
+  constexpr unsigned SB = sizeof (Sample);
+  const int row = Tl.nch * RQ;                                    // tap vectors per output group in the tap table
+  const unsigned qt_floats = (unsigned) NQ * row * 4, stage_floats = qt_floats + (unsigned) Tl.win * CB / (4 / SB);
+  __shared__ ArsBar s_full[2], s_empty[2];
+  __shared__ int s_rel[2][NO];
+  const int lane = threadIdx.x & 31;
+  const int warp = __shfl_sync (0xffffffffu, (int) (threadIdx.x >> 5), 0);
+  const int n_tiles = n_fb * n_cb;
+  if (threadIdx.x == 0) {
+    ars_bar_init (&s_full[0], ARS_PIPE_PROD); ars_bar_init (&s_full[1], ARS_PIPE_PROD);
+    ars_bar_init (&s_empty[0], NW); ars_bar_init (&s_empty[1], NW);
+#ifndef B200_CUDA_EMU
+    asm volatile ("fence.mbarrier_init.release.cluster;" ::: "memory");
+#endif
+  }
+  __syncthreads ();
+
+  // producing warps: positions of tile t's outputs, one bulk copy per tap row and per window row into stage b
+  auto produce = [&] (int t, int b) {
+    float *stage = smp + (size_t) b * stage_floats;
+    float4 *qt = (float4 *) stage;
+    float *xin = stage + qt_floats;
+    const int fb = t / n_cb, c_base = (t - fb * n_cb) * CB;
+    const long long o0 = (long long) fb * NO;
+    const int n_out = (int) min ((long long) NO, L.out_frames - o0);
+    long long f0; int ph0;
+    ars_position (L, o0, f0, ph0);
+    f0 &= ~3LL;
+#ifndef B200_CUDA_EMU
+    asm volatile ("fence.proxy.async.shared::cta;" ::: "memory");  // zero rows written two tiles ago vs this tile's bulk writes
+#endif
+    unsigned tx = 0;
+    if (lane < NO / ARS_PIPE_PROD) {
+      const int j = warp * (NO / ARS_PIPE_PROD) + lane;
+      long long idx; int phase;
+      ars_position (L, o0 + min (j, n_out - 1), idx, phase);
+      const int rel = (int) (idx - f0);
+      s_rel[b][j] = rel;
+      if ((j & (RQ - 1)) == 0) {
+        const float4 *src = Tl.qtab + ((size_t) (rel & 3) * L.out_step + phase) * row;
+        ars_bulk_g2s (qt + (size_t) (j / RQ) * row, src, (unsigned) row * 16u, &s_full[b]);
+        tx += (unsigned) row * 16u;
+      }
+    }
+    // a window that lies in the caller's input (every tile but the first few) is ONE tensor copy: box = CB channels x win
+    // frames, rows past the end of the input arrive as zeros (out-of-bounds fill) like the missing frames of the row path.
+    // (Divergent lanes issuing a bulk copy each are serialised through the uniform datapath: the row path below costs the
+    // producing warps ~40 copies each and makes them the tile's stragglers.)
+    const bool tensor = use_tm && f0 >= L.hist_frames;
+    if (tensor) {
+      if (warp == 0 && lane == 0) {
+        ars_tensor_g2s (xin, tm_in, c_base, (int) (f0 - L.hist_frames), &s_full[b]);
+        tx += (unsigned) Tl.win * CB * SB;
+      }
+    } else
+    for (int fr = warp + ARS_PIPE_PROD * lane; fr < Tl.win; fr += 32 * ARS_PIPE_PROD) {
+      const Sample *src = ars_frame_row<Sample> (L, f0 + fr);
+      float *dst = xin + (size_t) fr * (CB * SB / 4);
+      if (src) { ars_bulk_g2s (dst, src + c_base, CB * SB, &s_full[b]); tx += CB * SB; }
+      else {
+#pragma unroll 4
+        for (int i = 0; i < (int) (CB * SB / 16); i++) ((float4 *) dst)[i] = make_float4 (0.f, 0.f, 0.f, 0.f);
+      }
+    }
+#pragma unroll
+    for (int d = 16; d >= 1; d >>= 1) tx += __shfl_down_sync (0xffffffffu, tx, d);
+    ars_warp_sync ();                                             // the lanes' s_rel entries and zero rows before lane 0's release
+    if (lane == 0) ars_bar_arrive_tx (&s_full[b], tx);
+  };
+
+  int t = blockIdx.x, k = 0;
+  if (warp < ARS_PIPE_PROD && t < n_tiles) produce (t, 0);
+  for (; t < n_tiles; t += gridDim.x, k++) {
+    const int b = k & 1, tn = t + gridDim.x;
+    if (warp < ARS_PIPE_PROD && tn < n_tiles) {
+      if (k >= 1) ars_bar_wait (&s_empty[b ^ 1], (unsigned) ((k - 1) >> 1) & 1u);   // every warp is done with tile k - 1
+      produce (tn, b ^ 1);
+    }
+    ars_bar_wait (&s_full[b], (unsigned) (k >> 1) & 1u);
+
+    const typename S::Tap *qt = (const typename S::Tap *) (smp + (size_t) b * stage_floats);
+    const Sample *xin = (const Sample *) (smp + (size_t) b * stage_floats + qt_floats);
+    const int fb = t / n_cb;
+    const long long o0 = (long long) fb * NO;
+    const int n_out = (int) min ((long long) NO, L.out_frames - o0);
+    const int nq = (n_out + RQ - 1) / RQ;
+    const int c = (t - fb * n_cb) * CB + 4 * lane;
+    for (int q = warp; q < nq; q += NW) {
+      const int s_min = s_rel[b][q * RQ] & ~3;
+      const int s_max = (s_rel[b][min (q * RQ + RQ - 1, n_out - 1)] + L.n_taps + 3) & ~3;
+      S::group (L, xin + s_min * CB + 4 * lane, qt + (size_t) q * row, (s_max - s_min) >> 2, o0, q * RQ, c, n_out);
+    }
+    ars_warp_sync ();
+    if (lane == 0) ars_bar_arrive (&s_empty[b]);                  // this warp no longer reads stage b
+  }
+}
+
 __global__ void __launch_bounds__ (ARS_PIPE_THREADS, 1)
 ars_pipe_kernel (const ArsLaunch L, const ArsTile Tl, int n_fb, int n_cb, const __grid_constant__ ArsTensorMap tm_in, int use_tm)
 {
-  extern __shared__ __align__ (128) float smp[];
-  constexpr int RQ = ARS_RQ, NO = ARS_PIPE_NO, CB = ARS_PIPE_CB, NQ = NO / RQ, NW = ARS_PIPE_THREADS / 32;
-  const int row = Tl.nch * RQ;                                    // float4 per output group in the tap table
-  const unsigned qt_floats = (unsigned) NQ * row * 4, stage_floats = qt_floats + (unsigned) Tl.win * CB;
-  __shared__ ArsBar s_full[2], s_empty[2];
-  __shared__ int s_rel[2][NO];
-  const int lane = threadIdx.x & 31;
-  const int warp = __shfl_sync (0xffffffffu, (int) (threadIdx.x >> 5), 0);
-  const int n_tiles = n_fb * n_cb;
-  if (threadIdx.x == 0) {
-    ars_bar_init (&s_full[0], ARS_PIPE_PROD); ars_bar_init (&s_full[1], ARS_PIPE_PROD);
-    ars_bar_init (&s_empty[0], NW); ars_bar_init (&s_empty[1], NW);
-#ifndef B200_CUDA_EMU
-    asm volatile ("fence.mbarrier_init.release.cluster;" ::: "memory");
-#endif
-  }
-  __syncthreads ();
-
-  // producing warps: positions of tile t's outputs, one bulk copy per tap row and per window row into stage b
-  auto produce = [&] (int t, int b) {
-    float *stage = smp + (size_t) b * stage_floats;
-    float4 *qt = (float4 *) stage;
-    float *xin = stage + qt_floats;
-    const int fb = t / n_cb, c_base = (t - fb * n_cb) * CB;
-    const long long o0 = (long long) fb * NO;
-    const int n_out = (int) min ((long long) NO, L.out_frames - o0);
-    long long f0; int ph0;
-    ars_position (L, o0, f0, ph0);
-    f0 &= ~3LL;
-#ifndef B200_CUDA_EMU
-    asm volatile ("fence.proxy.async.shared::cta;" ::: "memory");  // zero rows written two tiles ago vs this tile's bulk writes
-#endif
-    unsigned tx = 0;
-    if (lane < NO / ARS_PIPE_PROD) {
-      const int j = warp * (NO / ARS_PIPE_PROD) + lane;
-      long long idx; int phase;
-      ars_position (L, o0 + min (j, n_out - 1), idx, phase);
-      const int rel = (int) (idx - f0);
-      s_rel[b][j] = rel;
-      if ((j & (RQ - 1)) == 0) {
-        const float4 *src = Tl.qtab + ((size_t) (rel & 3) * L.out_step + phase) * row;
-        ars_bulk_g2s (qt + (size_t) (j / RQ) * row, src, (unsigned) row * 16u, &s_full[b]);
-        tx += (unsigned) row * 16u;
-      }
-    }
-    // a window that lies in the caller's input (every tile but the first few) is ONE tensor copy: box = CB channels x win
-    // frames, rows past the end of the input arrive as zeros (out-of-bounds fill) like the missing frames of the row path.
-    // (Divergent lanes issuing a bulk copy each are serialised through the uniform datapath: the row path below costs the
-    // producing warps ~40 copies each and makes them the tile's stragglers.)
-    const bool tensor = use_tm && f0 >= L.hist_frames;
-    if (tensor) {
-      if (warp == 0 && lane == 0) {
-        ars_tensor_g2s (xin, &tm_in, c_base, (int) (f0 - L.hist_frames), &s_full[b]);
-        tx += (unsigned) Tl.win * CB * 4u;
-      }
-    } else
-    for (int fr = warp + ARS_PIPE_PROD * lane; fr < Tl.win; fr += 32 * ARS_PIPE_PROD) {
-      const long long f = f0 + fr;
-      const float *src = nullptr;
-      if (f < L.hist_frames) src = L.hist + f * L.channels;
-      else if (f < L.avail && L.in) src = L.in + (f - L.hist_frames) * L.channels;
-      float *dst = xin + (size_t) fr * CB;
-      if (src) { ars_bulk_g2s (dst, src + c_base, CB * 4u, &s_full[b]); tx += CB * 4u; }
-      else {
-#pragma unroll 4
-        for (int i = 0; i < CB / 4; i++) ((float4 *) dst)[i] = make_float4 (0.f, 0.f, 0.f, 0.f);
-      }
-    }
-#pragma unroll
-    for (int d = 16; d >= 1; d >>= 1) tx += __shfl_down_sync (0xffffffffu, tx, d);
-    ars_warp_sync ();                                             // the lanes' s_rel entries and zero rows before lane 0's release
-    if (lane == 0) ars_bar_arrive_tx (&s_full[b], tx);
-  };
-
-  int t = blockIdx.x, k = 0;
-  if (warp < ARS_PIPE_PROD && t < n_tiles) produce (t, 0);
-  for (; t < n_tiles; t += gridDim.x, k++) {
-    const int b = k & 1, tn = t + gridDim.x;
-    if (warp < ARS_PIPE_PROD && tn < n_tiles) {
-      if (k >= 1) ars_bar_wait (&s_empty[b ^ 1], (unsigned) ((k - 1) >> 1) & 1u);   // every warp is done with tile k - 1
-      produce (tn, b ^ 1);
-    }
-    ars_bar_wait (&s_full[b], (unsigned) (k >> 1) & 1u);
-
-    const float4 *qt = (const float4 *) (smp + (size_t) b * stage_floats);
-    const float *xin = smp + (size_t) b * stage_floats + qt_floats;
-    const int fb = t / n_cb;
-    const long long o0 = (long long) fb * NO;
-    const int n_out = (int) min ((long long) NO, L.out_frames - o0);
-    const int nq = (n_out + RQ - 1) / RQ;
-    const int c = (t - fb * n_cb) * CB + 4 * lane;
-    for (int q = warp; q < nq; q += NW) {
-      float acc[4][RQ][4];
-#pragma unroll
-      for (int u = 0; u < 4; u++)
-#pragma unroll
-        for (int r = 0; r < RQ; r++)
-#pragma unroll
-          for (int kk = 0; kk < 4; kk++) acc[u][r][kk] = 0.f;
-      const int s_min = s_rel[b][q * RQ] & ~3;
-      const int s_max = (s_rel[b][min (q * RQ + RQ - 1, n_out - 1)] + L.n_taps + 3) & ~3;
-      const int nch = (s_max - s_min) >> 2;
-      const float *xp = xin + s_min * CB + 4 * lane;
-      const float4 *tp = qt + (size_t) q * row;
-#pragma unroll 2
-      for (int ch = 0; ch < nch; ch++, xp += 4 * CB, tp += RQ) {
-        float x[4][4];
-#pragma unroll
-        for (int kk = 0; kk < 4; kk++) {
-          const float4 v = *(const float4 *) (xp + kk * CB);
-          x[0][kk] = v.x; x[1][kk] = v.y; x[2][kk] = v.z; x[3][kk] = v.w;
-        }
-#pragma unroll
-        for (int r = 0; r < RQ; r++) {
-          const float4 tq = tp[r];
-#pragma unroll
-          for (int u = 0; u < 4; u++) {
-            acc[u][r][0] = __fadd_rn (acc[u][r][0], __fmul_rn (x[u][0], tq.x));
-            acc[u][r][1] = __fadd_rn (acc[u][r][1], __fmul_rn (x[u][1], tq.y));
-            acc[u][r][2] = __fadd_rn (acc[u][r][2], __fmul_rn (x[u][2], tq.z));
-            acc[u][r][3] = __fadd_rn (acc[u][r][3], __fmul_rn (x[u][3], tq.w));
-          }
-        }
-      }
-      float *op = L.out + (size_t) (o0 + q * RQ) * L.channels + c;
-#pragma unroll
-      for (int r = 0; r < RQ; r++) {
-        if (q * RQ + r < n_out) {
-          float4 o;
-          o.x = __fadd_rn (__fadd_rn (acc[0][r][0], acc[0][r][2]), __fadd_rn (acc[0][r][1], acc[0][r][3]));
-          o.y = __fadd_rn (__fadd_rn (acc[1][r][0], acc[1][r][2]), __fadd_rn (acc[1][r][1], acc[1][r][3]));
-          o.z = __fadd_rn (__fadd_rn (acc[2][r][0], acc[2][r][2]), __fadd_rn (acc[2][r][1], acc[2][r][3]));
-          o.w = __fadd_rn (__fadd_rn (acc[3][r][0], acc[3][r][2]), __fadd_rn (acc[3][r][1], acc[3][r][3]));
-          *(float4 *) (op + (size_t) r * L.channels) = o;
-        }
-      }
-    }
-    ars_warp_sync ();
-    if (lane == 0) ars_bar_arrive (&s_empty[b]);                  // this warp no longer reads stage b
-  }
-}
-
-// sign-extending byte permute: the 16-bit sample in the low (0x9910) or high (0xbb32) half of a word as an int
-__device__ __forceinline__ int prmt_s16 (unsigned v, unsigned sel)
-{
-#ifdef B200_CUDA_EMU
-  return sel == 0x9910u ? (int) (short) (v & 0xffffu) : (int) (short) (v >> 16);
-#else
-  int d;
-  asm ("prmt.b32 %0, %1, 0, %2;" : "=r" (d) : "r" (v), "r" (sel));
-  return d;
-#endif
+  ars_pipe_body<ArsPipeF32> (L, Tl, n_fb, n_cb, &tm_in, use_tm);
 }
 
 // ---- ars_pipe_kernel_s16: the same pipeline for S16 streams ----------------------------------------------------------------
-// The window travels as raw 16-bit samples (one tensor copy of half the bytes), the tap rows as 32-bit ints in the F32 kernel's
-// chunk-major layout (host: ars_build_qtab_s16); a thread owns 4 channels x 4 outputs: per frame position one LDS.64 of samples
-// (4 sign-extending PRMT) and per output one broadcast LDS.128 of taps feed 16 IMAD - the IMADs (half rate) bound it exactly
-// where FMUL + FADD bound the F32 kernel.  Sums wrap in 32 bits, + 2^14, >> 15, saturate: byte-identical to ars_tile_kernel_s16.
+// The window travels as raw 16-bit samples (one tensor copy of half the bytes), the tap rows as 32-bit ints (ars_build_qtab
+// <int16_t, int32_t>); the IMADs (half rate) bound it exactly where FMUL + FADD bound the F32 kernel.  Sums wrap in 32 bits,
+// + 2^14, >> 15, saturate: byte-identical to ars_tile_kernel_s16.
 __global__ void __launch_bounds__ (ARS_PIPE_THREADS, 1)
 ars_pipe_kernel_s16 (const ArsLaunch L, const ArsTile Tl, int n_fb, int n_cb, const __grid_constant__ ArsTensorMap tm_in, int use_tm)
 {
-  extern __shared__ __align__ (128) float smp[];
-  constexpr int RQ = ARS_RQ, NO = ARS_PIPE_NO, CB = ARS_PIPE_CB, NQ = NO / RQ, NW = ARS_PIPE_THREADS / 32;
-  const int row = Tl.nch * RQ;                                    // float4 per output group in the tap table
-  // a stage = the tap rows (32-bit ints, the layout of the F32 kernel) + the window as RAW 16-bit samples (half a float each)
-  const unsigned qt_floats = (unsigned) NQ * row * 4, stage_floats = qt_floats + (unsigned) Tl.win * CB / 2;
-  const short *hist16 = (const short *) L.hist, *in16 = (const short *) L.in;
-  short *out16 = (short *) L.out;
-  __shared__ ArsBar s_full[2], s_empty[2];
-  __shared__ int s_rel[2][NO];
-  const int lane = threadIdx.x & 31;
-  const int warp = __shfl_sync (0xffffffffu, (int) (threadIdx.x >> 5), 0);
-  const int n_tiles = n_fb * n_cb;
-  if (threadIdx.x == 0) {
-    ars_bar_init (&s_full[0], ARS_PIPE_PROD); ars_bar_init (&s_full[1], ARS_PIPE_PROD);
-    ars_bar_init (&s_empty[0], NW); ars_bar_init (&s_empty[1], NW);
-#ifndef B200_CUDA_EMU
-    asm volatile ("fence.mbarrier_init.release.cluster;" ::: "memory");
-#endif
-  }
-  __syncthreads ();
-
-  // producing warps: positions of tile t's outputs, one bulk copy per tap row and per window row into stage b
-  auto produce = [&] (int t, int b) {
-    float *stage = smp + (size_t) b * stage_floats;
-    float4 *qt = (float4 *) stage;
-    float *xin = stage + qt_floats;
-    const int fb = t / n_cb, c_base = (t - fb * n_cb) * CB;
-    const long long o0 = (long long) fb * NO;
-    const int n_out = (int) min ((long long) NO, L.out_frames - o0);
-    long long f0; int ph0;
-    ars_position (L, o0, f0, ph0);
-    f0 &= ~3LL;
-#ifndef B200_CUDA_EMU
-    asm volatile ("fence.proxy.async.shared::cta;" ::: "memory");  // zero rows written two tiles ago vs this tile's bulk writes
-#endif
-    unsigned tx = 0;
-    if (lane < NO / ARS_PIPE_PROD) {
-      const int j = warp * (NO / ARS_PIPE_PROD) + lane;
-      long long idx; int phase;
-      ars_position (L, o0 + min (j, n_out - 1), idx, phase);
-      const int rel = (int) (idx - f0);
-      s_rel[b][j] = rel;
-      if ((j & (RQ - 1)) == 0) {
-        const float4 *src = Tl.qtab + ((size_t) (rel & 3) * L.out_step + phase) * row;
-        ars_bulk_g2s (qt + (size_t) (j / RQ) * row, src, (unsigned) row * 16u, &s_full[b]);
-        tx += (unsigned) row * 16u;
-      }
-    }
-    // a window that lies in the caller's input (every tile but the first few) is ONE tensor copy: box = CB channels x win
-    // frames, rows past the end of the input arrive as zeros (out-of-bounds fill) like the missing frames of the row path.
-    // (Divergent lanes issuing a bulk copy each are serialised through the uniform datapath: the row path below costs the
-    // producing warps ~40 copies each and makes them the tile's stragglers.)
-    const bool tensor = use_tm && f0 >= L.hist_frames;
-    if (tensor) {
-      if (warp == 0 && lane == 0) {
-        ars_tensor_g2s (xin, &tm_in, c_base, (int) (f0 - L.hist_frames), &s_full[b]);
-        tx += (unsigned) Tl.win * CB * 2u;
-      }
-    } else
-    for (int fr = warp + ARS_PIPE_PROD * lane; fr < Tl.win; fr += 32 * ARS_PIPE_PROD) {
-      const long long f = f0 + fr;
-      const short *src = nullptr;
-      if (f < L.hist_frames) src = hist16 + f * L.channels;
-      else if (f < L.avail && in16) src = in16 + (f - L.hist_frames) * L.channels;
-      float *dst = xin + (size_t) fr * (CB / 2);
-      if (src) { ars_bulk_g2s (dst, src + c_base, CB * 2u, &s_full[b]); tx += CB * 2u; }
-      else {
-#pragma unroll 4
-        for (int i = 0; i < CB / 8; i++) ((float4 *) dst)[i] = make_float4 (0.f, 0.f, 0.f, 0.f);
-      }
-    }
-#pragma unroll
-    for (int d = 16; d >= 1; d >>= 1) tx += __shfl_down_sync (0xffffffffu, tx, d);
-    ars_warp_sync ();                                             // the lanes' s_rel entries and zero rows before lane 0's release
-    if (lane == 0) ars_bar_arrive_tx (&s_full[b], tx);
-  };
-
-  int t = blockIdx.x, k = 0;
-  if (warp < ARS_PIPE_PROD && t < n_tiles) produce (t, 0);
-  for (; t < n_tiles; t += gridDim.x, k++) {
-    const int b = k & 1, tn = t + gridDim.x;
-    if (warp < ARS_PIPE_PROD && tn < n_tiles) {
-      if (k >= 1) ars_bar_wait (&s_empty[b ^ 1], (unsigned) ((k - 1) >> 1) & 1u);   // every warp is done with tile k - 1
-      produce (tn, b ^ 1);
-    }
-    ars_bar_wait (&s_full[b], (unsigned) (k >> 1) & 1u);
-
-    const int4 *qt = (const int4 *) (smp + (size_t) b * stage_floats);
-    const short *xin = (const short *) (smp + (size_t) b * stage_floats + qt_floats);
-    const int fb = t / n_cb;
-    const long long o0 = (long long) fb * NO;
-    const int n_out = (int) min ((long long) NO, L.out_frames - o0);
-    const int nq = (n_out + RQ - 1) / RQ;
-    const int c = (t - fb * n_cb) * CB + 4 * lane;
-    for (int q = warp; q < nq; q += NW) {
-      // integer sums wrap in 32 bits like the SSE2 pmaddwd path (inner_product_gint16_full_1_sse2, audio-resampler-x86-sse2.c:29-56):
-      // no lane structure to keep, one accumulator per (channel, output)
-      unsigned acc[4][RQ];
-#pragma unroll
-      for (int u = 0; u < 4; u++)
-#pragma unroll
-        for (int r = 0; r < RQ; r++) acc[u][r] = 0u;
-      const int s_min = s_rel[b][q * RQ] & ~3;
-      const int s_max = (s_rel[b][min (q * RQ + RQ - 1, n_out - 1)] + L.n_taps + 3) & ~3;
-      const int nch = (s_max - s_min) >> 2;
-      const short *xp = xin + s_min * CB + 4 * lane;
-      const int4 *tp = qt + (size_t) q * row;
-#pragma unroll 2
-      for (int ch = 0; ch < nch; ch++, xp += 4 * CB, tp += RQ) {
-        int x[4][4];
-#pragma unroll
-        for (int kk = 0; kk < 4; kk++) {
-          const uint2 v = *(const uint2 *) (xp + kk * CB);           // 4 adjacent channels of one frame, 16 bits each
-          x[0][kk] = prmt_s16 (v.x, 0x9910u); x[1][kk] = prmt_s16 (v.x, 0xbb32u);
-          x[2][kk] = prmt_s16 (v.y, 0x9910u); x[3][kk] = prmt_s16 (v.y, 0xbb32u);
-        }
-#pragma unroll
-        for (int r = 0; r < RQ; r++) {
-          const int4 tq = tp[r];
-#pragma unroll
-          for (int u = 0; u < 4; u++)
-            acc[u][r] += (unsigned) (x[u][0] * tq.x) + (unsigned) (x[u][1] * tq.y) + (unsigned) (x[u][2] * tq.z) + (unsigned) (x[u][3] * tq.w);
-        }
-      }
-      short *op = out16 + (size_t) (o0 + q * RQ) * L.channels + c;
-#pragma unroll
-      for (int r = 0; r < RQ; r++) {
-        if (q * RQ + r < n_out) {
-          // + 2^14, >> 15, saturate (audio-resampler-x86-sse2.c:48-54)
-          const int v0 = sat_s16 ((int) (acc[0][r] + (1u << 14)) >> 15), v1 = sat_s16 ((int) (acc[1][r] + (1u << 14)) >> 15);
-          const int v2 = sat_s16 ((int) (acc[2][r] + (1u << 14)) >> 15), v3 = sat_s16 ((int) (acc[3][r] + (1u << 14)) >> 15);
-          uint2 o;
-          o.x = ((unsigned) v0 & 0xffffu) | ((unsigned) v1 << 16);
-          o.y = ((unsigned) v2 & 0xffffu) | ((unsigned) v3 << 16);
-          *(uint2 *) (op + (size_t) r * L.channels) = o;
-        }
-      }
-    }
-    ars_warp_sync ();
-    if (lane == 0) ars_bar_arrive (&s_empty[b]);                  // this warp no longer reads stage b
-  }
+  ars_pipe_body<ArsPipeS16> (L, Tl, n_fb, n_cb, &tm_in, use_tm);
 }
 
+// S16 samples through the tile kernel's tiling: the window is staged widened to 32 bits, taps likewise; the sums are
+// integers (wrapping 32 bit like the SSE2 pmaddwd path), so no lane structure has to be kept —
+// inner_product_gint16_full_1_sse2 (audio-resampler-x86-sse2.c:29-56): sum, + 2^14, >> 15, saturate.
 template <int CB>
 __global__ void __launch_bounds__ (ARS_THREADS)
 ars_tile_kernel_s16 (const ArsLaunch L, const ArsTile Tl)
@@ -1236,7 +1103,7 @@ ars_tile_kernel_s16 (const ArsLaunch L, const ArsTile Tl)
   int4 *qt = (int4 *) sm;                                        // [nq][nch][RQ]
   int *xin = (int *) sm + (size_t) nq_max * Tl.nch * RQ * 4;      // [win][CB]
   __shared__ int s_rel[64], s_phase[64];
-  const short *hist = (const short *) L.hist, *in = (const short *) L.in, *phases = (const short *) L.phases;
+  const short *phases = (const short *) L.phases;
   short *out = (short *) L.out;
   const int lane = threadIdx.x & 31;
   const int warp = __shfl_sync (0xffffffffu, (int) (threadIdx.x >> 5), 0);
@@ -1254,10 +1121,7 @@ ars_tile_kernel_s16 (const ArsLaunch L, const ArsTile Tl)
   }
   const int c_base = blockIdx.y * CB;
   for (int fr = warp; fr < Tl.win; fr += ARS_THREADS / 32) {
-    const long long f = f0 + fr;
-    const short *src = nullptr;
-    if (f < L.hist_frames) src = hist + f * L.channels;
-    else if (f < L.avail && in) src = in + (f - L.hist_frames) * L.channels;
+    const short *src = ars_frame_row<short> (L, f0 + fr);
 #pragma unroll
     for (int c = lane; c < CB; c += 32)
       xin[fr * CB + c] = (src && c_base + c < L.channels) ? (int) __ldg (src + c_base + c) : 0;
@@ -1314,7 +1178,7 @@ ars_tile_kernel_s16 (const ArsLaunch L, const ArsTile Tl)
 #pragma unroll
       for (int u = 0; u < CPT; u++)
         if (q * RQ + r < n_out && c + u < L.channels)
-          out[(size_t) (o0 + q * RQ + r) * L.channels + c + u] = (short) sat_s16 ((int) (acc[u][r] + (1u << 14)) >> 15);
+          out[(size_t) (o0 + q * RQ + r) * L.channels + c + u] = (short) ars_round_s16 (acc[u][r]);
   }
 }
 
@@ -1385,7 +1249,7 @@ ars_interp_kernel (const ArsLaunch L, const float *__restrict__ table, int overs
       t[l] = __fadd_rn (__fadd_rn (__fmul_rn (acc[0][l], ic0), __fmul_rn (acc[1][l], ic1)),
           __fadd_rn (__fmul_rn (acc[2][l], ic2), __fmul_rn (acc[3][l], ic3)));
   if (live)
-    L.out[(size_t) o * L.channels + c] = __fadd_rn (__fadd_rn (t[0], t[2]), __fadd_rn (t[1], t[3]));
+    L.out[(size_t) o * L.channels + c] = ars_lane_sum (t);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1438,7 +1302,7 @@ ars_direct_kernel (const ArsLaunchX L)
     if (L.full) {                 // inner_product_gint16_full_1_sse2
       unsigned sum = 0;
       for (int i = 0; i < n; i++) sum += (unsigned) ((int) ars_sample<short> (L, idx + i, c) * (int) __ldg (tab + i));
-      ((short *) L.out)[(size_t) o * L.channels + c] = (short) sat_s16 ((int) (sum + (1u << 14)) >> 15);
+      ((short *) L.out)[(size_t) o * L.channels + c] = (short) ars_round_s16 (sum);
     } else if (LIN) {             // inner_product_gint16_linear_1_sse2 (audio-resampler-x86-sse2.c:57-108): 32-bit lane l
       unsigned s[2][4];           // sums the tap pairs (2l, 2l+1) of every eight; each LANE is shifted and multiplied
 #pragma unroll
@@ -1457,7 +1321,7 @@ ars_direct_kernel (const ArsLaunchX L)
 #pragma unroll
       for (int l = 0; l < 4; l++)
         acc += (unsigned) ((int) (short) ((int) s[0][l] >> 15) * x) + (unsigned) ((int) (short) ((int) s[1][l] >> 15) * y);
-      ((short *) L.out)[(size_t) o * L.channels + c] = (short) sat_s16 ((int) (acc + (1u << 14)) >> 15);
+      ((short *) L.out)[(size_t) o * L.channels + c] = (short) ars_round_s16 (acc);
     } else {                      // inner_product_gint16_cubic_1_sse2
       unsigned s0 = 0, s1 = 0, s2 = 0, s3 = 0;
       for (int i = 0; i < n; i++) {
@@ -1471,14 +1335,14 @@ ars_direct_kernel (const ArsLaunchX L)
       cubic_coeff_s16 (frac, L.out_step, ic);
       const unsigned acc = (unsigned) ((int) (short) ((int) s0 >> 15) * ic[0]) + (unsigned) ((int) (short) ((int) s1 >> 15) * ic[1]) +
           (unsigned) ((int) (short) ((int) s2 >> 15) * ic[2]) + (unsigned) ((int) (short) ((int) s3 >> 15) * ic[3]);
-      ((short *) L.out)[(size_t) o * L.channels + c] = (short) sat_s16 ((int) (acc + (1u << 14)) >> 15);
+      ((short *) L.out)[(size_t) o * L.channels + c] = (short) ars_round_s16 (acc);
     }
   } else if (FMT == ARS_S32) {
     const int *tab = (const int *) L.table + row0;
     if (L.full) {                 // inner_product_gint32_full_1_sse41
       unsigned long long sum = 0;
       for (int i = 0; i < n; i++) sum += (unsigned long long) ((long long) ars_sample<int> (L, idx + i, c) * __ldg (tab + i));
-      ((int *) L.out)[(size_t) o * L.channels + c] = (int) sat_s32 (((long long) sum + (1 << 30)) >> 31);
+      ((int *) L.out)[(size_t) o * L.channels + c] = ars_round_s32 (sum);
     } else {                      // inner_product_gint32_cubic_1_sse41: each 64-bit LANE (even / odd taps) is
       unsigned long long s[4][2]; // shifted and multiplied before the lanes are added; _linear_1_sse41 (:70-112) is the same
       constexpr int ROWS = LIN ? 2 : 4;   // arithmetic over two rows
@@ -1504,7 +1368,7 @@ ars_direct_kernel (const ArsLaunchX L)
 #pragma unroll
         for (int l = 0; l < 2; l++)
           acc += (unsigned long long) ((long long) (int) (unsigned) (s[k][l] >> 31) * (long long) ic[k]);
-      ((int *) L.out)[(size_t) o * L.channels + c] = (int) sat_s32 (((long long) acc + (1 << 30)) >> 31);
+      ((int *) L.out)[(size_t) o * L.channels + c] = ars_round_s32 (acc);
     }
   } else {
     const double *tab = (const double *) L.table + row0;
@@ -1582,13 +1446,13 @@ ars_small_kernel (const ArsLaunchX L, int nearest)
     const short *tab = (const short *) L.table + row0;
     unsigned sum = 0;
     for (int i = 0; i < n; i++) sum += (unsigned) ((int) ars_sample<short> (L, idx + i, c) * (int) __ldg (tab + i));
-    ((short *) L.out)[at] = (short) sat_s16 ((int) (sum + (1u << 14)) >> 15);
+    ((short *) L.out)[at] = (short) ars_round_s16 (sum);
   } else if (FMT == ARS_S32) {
     if (nearest) { ((int *) L.out)[at] = ars_sample<int> (L, idx, c); return; }
     const int *tab = (const int *) L.table + row0;
     unsigned long long sum = 0;
     for (int i = 0; i < n; i++) sum += (unsigned long long) ((long long) ars_sample<int> (L, idx + i, c) * __ldg (tab + i));
-    ((int *) L.out)[at] = (int) sat_s32 (((long long) sum + (1 << 30)) >> 31);
+    ((int *) L.out)[at] = ars_round_s32 (sum);
   } else if (FMT == ARS_F64) {
     if (nearest) { ((double *) L.out)[at] = ars_sample<double> (L, idx, c); return; }
     const double *tab = (const double *) L.table + row0;
@@ -1606,13 +1470,13 @@ ars_small_kernel (const ArsLaunchX L, int nearest)
 #pragma unroll
       for (int l = 0; l < 4; l++)
         if (i + l < n) s[l] = __fadd_rn (s[l], __fmul_rn (ars_sample<float> (L, idx + i + l, c), __ldg (tab + i + l)));
-    ((float *) L.out)[at] = __fadd_rn (__fadd_rn (s[0], s[2]), __fadd_rn (s[1], s[3]));
+    ((float *) L.out)[at] = ars_lane_sum (s);
   }
 }
 
 // new history = frames [first, first+keep) of the (old history ++ input) stream, any sample width
 template <typename T>
-__global__ void ars_history_kernel_x (T *dst, const T *hist, const T *in, long long hist_frames,
+__device__ __forceinline__ void ars_history_copy (T *dst, const T *hist, const T *in, long long hist_frames,
     long long first, long long keep, int channels)
 {
   const long long n = keep * channels;
@@ -1626,19 +1490,16 @@ __global__ void ars_history_kernel_x (T *dst, const T *hist, const T *in, long l
   }
 }
 
-// new history = frames [first, first+keep) of the (old history ++ input) stream
-__global__ void ars_history_kernel (float *dst, const float *hist, const float *in, long long hist_frames,
-    long long first, long long keep, int channels)
+// the kernels keep their names (F32 and S32 samples: ars_history_kernel), which the launch records pin
+template <typename T>
+__global__ void ars_history_kernel_x (T *dst, const T *hist, const T *in, long long hist_frames, long long first, long long keep, int channels)
 {
-  const long long n = keep * channels;
-  for (long long i = blockIdx.x * (long long) blockDim.x + threadIdx.x; i < n; i += (long long) gridDim.x * blockDim.x) {
-    const long long f = first + i / channels;
-    const int c = (int) (i % channels);
-    float v = 0.f;
-    if (f < hist_frames) v = hist[f * channels + c];
-    else if (in) v = in[(f - hist_frames) * channels + c];
-    dst[i] = v;
-  }
+  ars_history_copy (dst, hist, in, hist_frames, first, keep, channels);
+}
+__global__ void ars_history_kernel (float *dst, const float *hist, const float *in, long long hist_frames, long long first, long long keep,
+    int channels)
+{
+  ars_history_copy (dst, hist, in, hist_frames, first, keep, channels);
 }
 
 }  // namespace b200
@@ -1821,8 +1682,9 @@ static int ars_upload_tables (b200_ars * h)
   // layout) for its pipeline; bounded by the FULL-mode threshold (bps * n_taps * out_rate < 1 MiB  =>  at most 16 x that)
   if (st == B200_OK && q.full && !q.small && !q.copy && (q.fmt == ARS_F32 || (q.fmt == ARS_S16 && (q.channels % ARS_PIPE_CB) == 0))) {
     std::vector<float> tab;
-    if (q.fmt == ARS_F32) ars_build_qtab (q, ars_tile_geometry (q, 0).nch, &tab);
-    else ars_build_qtab_s16 (q, ars_tile_geometry (q, 0).nch, &tab);
+    const int nch = ars_tile_geometry (q, 0).nch;
+    if (q.fmt == ARS_F32) ars_build_qtab<float, float> (q, q.phases.data (), nch, &tab);
+    else ars_build_qtab<int16_t, int32_t> (q, (const int16_t *) q.phases_x.data (), nch, &tab);
     st = upload (&h->d_qtab, tab.data (), tab.size ());
   }
   return st;

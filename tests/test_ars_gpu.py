@@ -146,15 +146,30 @@ def test_interpolated_filter_mode(cuda_device, cfg):
     _stream_through(a, b, ch, q, [480, 480, 100, 1, 2000, 37], seed=ch)
 
 
+# the F32 knob sets that reach the other kernels sharing the F32 group inner product: ars_pipe_kernel_v1 and the tile
+# kernels <128, 4>, <128, 1>, <64, 1>
+PIPELINE_KNOBS = [None, "B200_ARS_PIPE_V1=1", "B200_ARS_NOPIPE=1 B200_ARS_CPT=4", "B200_ARS_NOPIPE=1 B200_ARS_CPT=1",
+                  "B200_ARS_NOPIPE=1 B200_ARS_CB=64 B200_ARS_CPT=1"]
+PIPELINE_CASES = [("F32", k) for k in PIPELINE_KNOBS] + [("S16", None)]
+
+
+def pipeline_case_id(case):
+    fmt, knob = case
+    return fmt if knob is None else "%s-%s" % (fmt, knob.replace(" ", "-"))
+
+
 @pytest.mark.parametrize("grid", ["3", "16"])
-@pytest.mark.parametrize("fmt", ["F32", "S16"])
-def test_pipeline_many_tiles_per_cta(cuda_device, monkeypatch, fmt, grid):
+@pytest.mark.parametrize("fmt,knobs", PIPELINE_CASES, ids=[pipeline_case_id(c) for c in PIPELINE_CASES])
+def test_pipeline_many_tiles_per_cta(cuda_device, monkeypatch, fmt, knobs, grid):
     """the persistent pipelines (ars_pipe_kernel, ars_pipe_kernel_s16) with FEWER CTAs than tiles (B200_ARS_GRID): every CTA walks
     dozens of tiles through its two stages - full / empty barrier phases, the tensor-copy path and the row path of the tiles that
-    touch the history, a last partial tile - byte-identical to the oracle over several buffers"""
+    touch the history, a last partial tile - byte-identical to the oracle over several buffers; under the knob sets the same
+    streams through ars_pipe_kernel_v1 and the tile kernels"""
     import torch
     from gstreamer_b200.audio import CudaAudioResample
     monkeypatch.setenv("B200_ARS_GRID", grid)
+    for kv in (knobs or "").split():
+        monkeypatch.setenv(*kv.split("="))
     a, b, ch, q = 48000, 44100, 256, 4
     ofmt, gfmt, dt, _ = ob.AUDIO_FORMATS[fmt]
     o = ob.oracle()

@@ -517,12 +517,27 @@ def test_audio_kernels(emu, fmt, opts, monkeypatch):
             o.oracle_ars_free(ho)
 
 
-@pytest.mark.parametrize("fmt", ["F32", "S16"])
-def test_audio_pipeline_many_tiles_per_cta(emu, monkeypatch, fmt):
+# the F32 knob sets that reach the other kernels sharing the F32 group inner product: ars_pipe_kernel_v1 and the tile
+# kernels <128, 4>, <128, 1>, <64, 1>
+PIPELINE_KNOBS = [None, "B200_ARS_PIPE_V1=1", "B200_ARS_NOPIPE=1 B200_ARS_CPT=4", "B200_ARS_NOPIPE=1 B200_ARS_CPT=1",
+                  "B200_ARS_NOPIPE=1 B200_ARS_CB=64 B200_ARS_CPT=1"]
+PIPELINE_CASES = [("F32", k) for k in PIPELINE_KNOBS] + [("S16", None)]
+
+
+def pipeline_case_id(case):
+    fmt, knob = case
+    return fmt if knob is None else "%s-%s" % (fmt, knob.replace(" ", "-"))
+
+
+@pytest.mark.parametrize("fmt,knobs", PIPELINE_CASES, ids=[pipeline_case_id(c) for c in PIPELINE_CASES])
+def test_audio_pipeline_many_tiles_per_cta(emu, monkeypatch, fmt, knobs):
     """ars_pipe_kernel's stage hand-over (full / empty barriers, two stages): B200_ARS_GRID=2 makes each persistent CTA walk
-    a dozen tiles, with start-up zeros, a silent call (no input pointer) and a last partial tile"""
+    a dozen tiles, with start-up zeros, a silent call (no input pointer) and a last partial tile; under the knob sets the
+    same streams through ars_pipe_kernel_v1 and the tile kernels"""
     from gstreamer_b200 import _lib
     monkeypatch.setenv("B200_ARS_GRID", "2")
+    for kv in (knobs or "").split():
+        monkeypatch.setenv(*kv.split("="))
     ofmt, gfmt, dt, _ = ob.AUDIO_FORMATS[fmt]
     o = ob.oracle()
     for (a, b, ch, grid) in [(48000, 44100, 256, "2"), (44100, 48000, 128, "3"), (48000, 44100, 128, "1")]:
