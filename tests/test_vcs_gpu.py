@@ -22,8 +22,7 @@ SIZES = [
 METHODS = list(range(10))
 
 
-def _run_gpu(iw, ih, ow, oh, method, frame, in_fmt=23, out_fmt=12, site=None, matrix=None, rng=None,
-             batch=1):
+def _run_gpu(iw, ih, ow, oh, method, frame, in_fmt=23, out_fmt=12, site=None, matrix=None, rng=None):
     import torch
     import gstreamer_b200 as g
     el = g.CudaVideoConvertScale(add_borders=False, method=method, cuda_device_id=0)
@@ -32,14 +31,10 @@ def _run_gpu(iw, ih, ow, oh, method, frame, in_fmt=23, out_fmt=12, site=None, ma
     oi = g.VideoInfo(out_fmt, ow, oh)
     el.set_info(ii, oi)
     assert ii.size == frame.size
-    src = [torch.from_numpy(frame).cuda() for _ in range(batch)]
-    dst = [torch.full((oi.size,), 0xA5, dtype=torch.uint8, device="cuda") for _ in range(batch)]
-    if batch == 1:
-        el.transform_frame(src[0], dst[0])
-    else:
-        el.transform_frames(src, dst)
+    dst = torch.full((oi.size,), 0xA5, dtype=torch.uint8, device="cuda")
+    el.transform_frame(torch.from_numpy(frame).cuda(), dst)
     torch.cuda.synchronize()
-    return [d.cpu().numpy() for d in dst]
+    return [dst.cpu().numpy()]
 
 
 @pytest.mark.parametrize("size", SIZES, ids=lambda s: "%dx%d-%dx%d" % s)
@@ -87,15 +82,6 @@ def test_baseline_configs_full_size(cuda_device, cfg, content):
     got = _run_gpu(iw, ih, ow, oh, method, frame)[0]
     bad = np.nonzero(got != want)[0]
     assert bad.size == 0, f"{bad.size} bytes differ, first at {bad[:8]}"
-
-
-def test_batch_equals_single(cuda_device):
-    iw, ih, ow, oh = 642, 362, 320, 180
-    frame = ob.nv12_random_frame(iw, ih, 11)
-    single = _run_gpu(iw, ih, ow, oh, 3, frame)[0]
-    many = _run_gpu(iw, ih, ow, oh, 3, frame, batch=5)
-    for m in many:
-        assert np.array_equal(m, single)
 
 
 def test_custom_strides_and_offsets(cuda_device):

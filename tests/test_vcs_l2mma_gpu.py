@@ -14,7 +14,8 @@ SIZES = [(16, 16), (64, 48), (256, 144), (496, 272), (1920, 1088), (3840, 2160)]
 METHODS = [3, 5, 6, 7, 8, 9]
 
 
-def convert(iw, ih, method, frame, in_fmt=23, out_fmt=12, matrix=None, rng=None, batch=1):
+def convert(iw, ih, method, frames, in_fmt=23, out_fmt=12, matrix=None, rng=None):
+    """one frame, or a batch (a list of frames) in one transform_frames call"""
     import torch
     import gstreamer_b200 as g
     el = g.CudaVideoConvertScale(add_borders=False, method=method)
@@ -23,9 +24,9 @@ def convert(iw, ih, method, frame, in_fmt=23, out_fmt=12, matrix=None, rng=None,
     el.set_info(ii, oi)
     el.set_kernel_variant(6)
     assert el.plan_info().kernel_variant == 6
-    src = [torch.from_numpy(frame).cuda() for _ in range(batch)]
-    dst = [torch.full((oi.size,), 0x5A, dtype=torch.uint8, device="cuda") for _ in range(batch)]
-    if batch == 1:
+    src = [torch.from_numpy(f).cuda() for f in (frames if isinstance(frames, list) else [frames])]
+    dst = [torch.full((oi.size,), 0x5A, dtype=torch.uint8, device="cuda") for _ in src]
+    if len(src) == 1:
         el.transform_frame(src[0], dst[0])
     else:
         el.transform_frames(src, dst)
@@ -51,7 +52,6 @@ def test_tensor_path_matches_oracle(cuda_device, size, method):
 def test_tensor_path_formats_and_batch(cuda_device, in_fmt, out_fmt):
     iw, ih = 496, 272
     d = ob.vcs_desc(iw, ih, iw // 2, ih // 2, 3, in_fmt=ob.FMT[in_fmt], out_fmt=ob.FMT[out_fmt], site=2, matrix=4, rng=1)
-    frame = ob.nv12_random_frame(iw, ih, seed=3)
-    want = ob.oracle_vcs_convert(d, frame)
-    for got in convert(iw, ih, 3, frame, ob.FMT[in_fmt], ob.FMT[out_fmt], matrix=4, rng=1, batch=3):
-        assert np.array_equal(got, want)
+    frames = [ob.nv12_random_frame(iw, ih, seed=3 + k) for k in range(3)]          # a frame of its own in every slot
+    for k, got in enumerate(convert(iw, ih, 3, frames, ob.FMT[in_fmt], ob.FMT[out_fmt], matrix=4, rng=1)):
+        assert np.array_equal(got, ob.oracle_vcs_convert(d, frames[k])), f"frame {k}"

@@ -15,7 +15,8 @@ SIZES = [(32, 16), (256, 56), (272, 64), (512, 240), (1024, 448), (1936, 1096), 
 METHODS = [3, 5, 6, 7, 8, 9]
 
 
-def convert(iw, ih, method, frame, in_fmt=23, out_fmt=12, matrix=None, rng=None, batch=1):
+def convert(iw, ih, method, frames, in_fmt=23, out_fmt=12, matrix=None, rng=None):
+    """one frame, or a batch (a list of frames) in one transform_frames call"""
     import torch
     import gstreamer_b200 as g
     el = g.CudaVideoConvertScale(add_borders=False, method=method)
@@ -24,9 +25,9 @@ def convert(iw, ih, method, frame, in_fmt=23, out_fmt=12, matrix=None, rng=None,
     el.set_info(ii, oi)
     el.set_kernel_variant(7)
     assert el.plan_info().kernel_variant == 7
-    src = [torch.from_numpy(frame).cuda() for _ in range(batch)]
-    dst = [torch.full((oi.size,), 0x5A, dtype=torch.uint8, device="cuda") for _ in range(batch)]
-    if batch == 1:
+    src = [torch.from_numpy(f).cuda() for f in (frames if isinstance(frames, list) else [frames])]
+    dst = [torch.full((oi.size,), 0x5A, dtype=torch.uint8, device="cuda") for _ in src]
+    if len(src) == 1:
         el.transform_frame(src[0], dst[0])
     else:
         el.transform_frames(src, dst)
@@ -50,10 +51,10 @@ def test_matches_oracle(cuda_device, size, method):
 @pytest.mark.parametrize("in_fmt,out_fmt", [("NV21", "BGRA"), ("NV12", "RGBA"), ("NV21", "xRGB"), ("NV12", "ABGR")])
 def test_formats_and_batches(cuda_device, in_fmt, out_fmt):
     iw, ih = 528, 136
-    frame = ob.nv12_random_frame(iw, ih, seed=3)
-    want = ob.oracle_vcs_convert(ob.vcs_desc(iw, ih, iw // 2, ih // 2, 3, in_fmt=ob.FMT[in_fmt], out_fmt=ob.FMT[out_fmt], site=2), frame)
-    for got in convert(iw, ih, 3, frame, in_fmt=ob.FMT[in_fmt], out_fmt=ob.FMT[out_fmt], batch=5):
-        assert np.array_equal(got, want)
+    frames = [ob.nv12_random_frame(iw, ih, seed=3 + k) for k in range(5)]          # a frame of its own in every slot
+    d = ob.vcs_desc(iw, ih, iw // 2, ih // 2, 3, in_fmt=ob.FMT[in_fmt], out_fmt=ob.FMT[out_fmt], site=2)
+    for k, got in enumerate(convert(iw, ih, 3, frames, in_fmt=ob.FMT[in_fmt], out_fmt=ob.FMT[out_fmt])):
+        assert np.array_equal(got, ob.oracle_vcs_convert(d, frames[k])), f"frame {k}"
 
 
 @pytest.mark.parametrize("matrix,rng", [(3, 2), (4, 1), (6, 2)])

@@ -25,7 +25,7 @@ def rgb_frame(iw, ih, seed):
     return np.random.default_rng(seed).integers(0, 256, iw * ih * 4, dtype=np.uint8)
 
 
-def convert(size, method, frame, fi, fo, colorimetry=None, batch=1):
+def convert(size, method, frame, fi, fo, colorimetry=None):
     import torch
     import gstreamer_b200 as g
     iw, ih, ow, oh = size
@@ -35,14 +35,10 @@ def convert(size, method, frame, fi, fo, colorimetry=None, batch=1):
         oi.set_colorimetry(matrix=colorimetry[0], range=colorimetry[1], chroma_site=colorimetry[2])
     el.set_info(ii, oi)
     assert int(el.plan_info().kernel_variant) == 5
-    src = [torch.from_numpy(frame).cuda() for _ in range(batch)]
-    dst = [torch.full((oi.size,), 0x5A, dtype=torch.uint8, device="cuda") for _ in range(batch)]
-    if batch == 1:
-        el.transform_frame(src[0], dst[0])
-    else:
-        el.transform_frames(src, dst)
+    dst = torch.full((oi.size,), 0x5A, dtype=torch.uint8, device="cuda")
+    el.transform_frame(torch.from_numpy(frame).cuda(), dst)
     torch.cuda.synchronize()
-    return [d.cpu().numpy() for d in dst], oi
+    return [dst.cpu().numpy()], oi
 
 
 def expected(size, method, frame, fi, fo, colorimetry=None):
@@ -78,16 +74,6 @@ def test_rgb_to_420_colorimetry(cuda_device, colorimetry):
         want = expected(size, 3, frame, "BGRA", "NV12", colorimetry)
         (got,), oi = convert(size, 3, frame, "BGRA", "NV12", colorimetry)
         assert not planes_equal(got, want, oi, size[2], size[3], True)
-
-
-def test_rgb_to_420_batch(cuda_device):
-    from test_vcs_cross_gpu import planes_equal
-    size = (640, 360, 426, 240)
-    frame = rgb_frame(640, 360, 9)
-    want = expected(size, 1, frame, "RGBA", "I420")
-    outs, oi = convert(size, 1, frame, "RGBA", "I420", batch=4)
-    for o in outs:
-        assert not planes_equal(o, want, oi, 426, 240, False)
 
 
 @pytest.mark.parametrize("method", [0, 1, 3, 4, 9], ids=["nearest", "bilinear", "lanczos", "bilinear2", "mitchell"])

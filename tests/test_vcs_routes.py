@@ -17,6 +17,12 @@ import make_vcs_routes as mr  # noqa: E402
 
 pytestmark = pytest.mark.timeout(600)
 
+# every kernel a convert launches (tests/vcs_batch_cases.py runs each of them on batches of distinct frames)
+GRID_KERNELS = {"vcs_border_kernel", "vcs_down420_kernel", "vcs_generic_kernel", "vcs_l2mma_kernel", "vcs_lanczos2_kernel",
+                "vcs_lanczos2_v2_kernel", "vcs_light_kernel", "vcs_ntap_kernel", "vcs_ntap_vfirst_kernel", "vcs_planes_fast_kernel",
+                "vcs_planes_fast_vfirst_kernel", "vcs_planes_kernel", "vcs_planes_vec_kernel", "vcs_rgb2ayuv_kernel",
+                "vcs_rgb420_kernel", "vcs_rgb_deinterleave_kernel", "vcs_yuy2_420_kernel", "vcs_yuy2_ayuv_kernel"}
+
 # kernel_name -> the launched kernels it stands for: the n-tap launcher picks its vertical-first form where that is
 # cheaper, the plane launcher runs copy / halve planes through vcs_planes_vec_kernel
 NAMED = {"vcs_ntap_kernel": {"vcs_ntap_kernel", "vcs_ntap_vfirst_kernel"},
@@ -42,11 +48,7 @@ def test_routes_match_fixture(routes, knob):
 def test_grid_reaches_every_kernel(routes):
     got, _ = routes
     launched = {re.sub(r"<.*", "", x) for x in got["launches"] for x in x}
-    assert launched == {"vcs_border_kernel", "vcs_down420_kernel", "vcs_generic_kernel", "vcs_l2mma_kernel",
-                        "vcs_lanczos2_kernel", "vcs_lanczos2_v2_kernel", "vcs_light_kernel", "vcs_ntap_kernel",
-                        "vcs_ntap_vfirst_kernel", "vcs_planes_fast_kernel", "vcs_planes_fast_vfirst_kernel",
-                        "vcs_planes_kernel", "vcs_planes_vec_kernel", "vcs_rgb2ayuv_kernel", "vcs_rgb420_kernel",
-                        "vcs_rgb_deinterleave_kernel", "vcs_yuy2_420_kernel", "vcs_yuy2_ayuv_kernel"}
+    assert launched == GRID_KERNELS
 
 
 @pytest.mark.parametrize("knob", [None] + mr.KNOBS)
