@@ -10,6 +10,9 @@ typedef struct _GstAudioInfo { const GstAudioFormatInfo *finfo; guint flags; gin
 #define GST_AUDIO_INFO_BPF(i) ((i)->bpf)
 #define GST_AUDIO_INFO_FORMAT(i) ((i)->finfo->format)
 #define GST_AUDIO_NE(s) #s "LE"
+#define GST_AUDIO_FORMATS_ALL "{ F64LE, F64BE, F32LE, F32BE, S32LE, S32BE, U32LE, U32BE, S24_32LE, S24_32BE, U24_32LE, " \
+    "U24_32BE, S24LE, S24BE, U24LE, U24BE, S20_32LE, S20_32BE, U20_32LE, U20_32BE, S20LE, S20BE, U20LE, U20BE, S18LE, " \
+    "S18BE, U18LE, U18BE, S16LE, S16BE, U16LE, U16BE, S8, U8 }"
 gboolean gst_audio_info_from_caps (GstAudioInfo * info, const GstCaps * caps);
 enum { GST_AUDIO_RESAMPLER_METHOD_NEAREST, GST_AUDIO_RESAMPLER_METHOD_LINEAR, GST_AUDIO_RESAMPLER_METHOD_CUBIC,
   GST_AUDIO_RESAMPLER_METHOD_BLACKMAN_NUTTALL, GST_AUDIO_RESAMPLER_METHOD_KAISER };

@@ -19,8 +19,8 @@
 GST_DEBUG_CATEGORY_STATIC (cuda_ars_debug);
 #define GST_CAT_DEFAULT cuda_ars_debug
 
-#define ARS_CAPS "audio/x-raw, format = (string) { " GST_AUDIO_NE (F32) ", " GST_AUDIO_NE (S16) ", " GST_AUDIO_NE (S32) ", " \
-    GST_AUDIO_NE (F64) " }, layout = (string) interleaved, " \
+/* every sample format, as the stock element (gstaudioresample.c:84-85); interleaved only */
+#define ARS_CAPS "audio/x-raw, format = (string) " GST_AUDIO_FORMATS_ALL ", layout = (string) interleaved, " \
     "rate = (int) [ 1, MAX ], channels = (int) [ 1, MAX ]"
 static GstStaticPadTemplate ars_sink = GST_STATIC_PAD_TEMPLATE ("sink", GST_PAD_SINK, GST_PAD_ALWAYS, GST_STATIC_CAPS (ARS_CAPS));
 static GstStaticPadTemplate ars_src = GST_STATIC_PAD_TEMPLATE ("src", GST_PAD_SRC, GST_PAD_ALWAYS, GST_STATIC_CAPS (ARS_CAPS));

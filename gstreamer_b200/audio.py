@@ -15,9 +15,23 @@ from .video import _ptr, _stream
 
 
 class AudioFormat:
-    """GstAudioFormat values of the sample formats the element resamples natively (audio-converter.c:700-727)"""
-    S16LE, S32LE, F32LE, F64LE = 4, 12, 28, 30
+    """GstAudioFormat values of every interleaved sample format the element resamples.  S16LE, S32LE, F32LE and F64LE are
+    resampled as they are (audio-converter.c:700-727); the others are unpacked to S32 or F64 inside the kernels and
+    quantized and packed back on store."""
+    S8, U8, S16LE, S16BE, U16LE, U16BE = 2, 3, 4, 5, 6, 7
+    S24_32LE, S24_32BE, U24_32LE, U24_32BE, S32LE, S32BE, U32LE, U32BE = 8, 9, 10, 11, 12, 13, 14, 15
+    S24LE, S24BE, U24LE, U24BE, S20LE, S20BE, U20LE, U20BE, S18LE, S18BE, U18LE, U18BE = range(16, 28)
+    F32LE, F32BE, F64LE, F64BE = 28, 29, 30, 31
+    S20_32LE, S20_32BE, U20_32LE, U20_32BE = 32, 33, 34, 35
     DTYPE = {4: np.int16, 12: np.int32, 28: np.float32, 30: np.float64}
+    # bytes per sample in a buffer (GST_AUDIO_FORMAT_INFO_WIDTH / 8)
+    WIDTH = {2: 1, 3: 1, 4: 2, 5: 2, 6: 2, 7: 2, **{v: 4 for v in range(8, 16)}, **{v: 3 for v in range(16, 28)},
+             28: 4, 29: 4, 30: 8, 31: 8, 32: 4, 33: 4, 34: 4, 35: 4}
+    NAMES = {2: "S8", 3: "U8", 4: "S16LE", 5: "S16BE", 6: "U16LE", 7: "U16BE", 8: "S24_32LE", 9: "S24_32BE", 10: "U24_32LE",
+             11: "U24_32BE", 12: "S32LE", 13: "S32BE", 14: "U32LE", 15: "U32BE", 16: "S24LE", 17: "S24BE", 18: "U24LE",
+             19: "U24BE", 20: "S20LE", 21: "S20BE", 22: "U20LE", 23: "U20BE", 24: "S18LE", 25: "S18BE", 26: "U18LE",
+             27: "U18BE", 28: "F32LE", 29: "F32BE", 30: "F64LE", 31: "F64BE", 32: "S20_32LE", 33: "S20_32BE",
+             34: "U20_32LE", 35: "U20_32BE"}
 
 
 class CudaAudioResample:

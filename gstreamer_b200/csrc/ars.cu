@@ -58,6 +58,20 @@ static double bessel_i0 (double x)
   return y;
 }
 
+// The caller's samples of a format the resampler does not work in (converter_generic, audio-converter.c:1281-1310): each
+// is unpacked on load (do_unpack with GST_AUDIO_PACK_FLAG_TRUNCATE_RANGE, :455-490) and quantized and packed on store
+// (chain_quantize :968-1021, pack flags 0 :1305).  Warp-uniform: one descriptor per launch.
+enum ArsIoKind : int { ARS_IO_NONE = 0, ARS_IO_INT = 1, ARS_IO_F32 = 2, ARS_IO_F64 = 3 };
+struct ArsIo {
+  int kind;                      // ArsIoKind: integer -> S32, F32BE -> F64, F64BE -> F64
+  int step;                      // bytes from one sample to the next
+  int big;                       // big-endian bytes
+  int shift;                     // integer formats: 32 - depth (unpack shifts left, pack right)
+  int arith;                     // pack shifts arithmetically (signed 4-byte formats: shrsl of pack_s24_32)
+  int qshift;                    // quantize to depth bits (32 - depth) or 0 (32-bit formats)
+  unsigned sign;                 // 0x80000000 for unsigned formats
+};
+
 struct ArsPlan {
   int channels = 0, in_step = 0, out_step = 0;   // rates / gcd
   int samp_inc = 0, samp_frac = 0;
@@ -73,11 +87,37 @@ struct ArsPlan {
   std::vector<float> proto;      // (oversample + isize) x n_taps oversampled prototype
   std::vector<float> phases;     // n_phases x n_taps (FULL mode), all phases precomputed
   // other sample formats: the same two tables in the samples' own type
-  int fmt = 0, bps = 4;          // ArsFmt, bytes per sample
+  int fmt = 0, bps = 4;          // ArsFmt, bytes per sample: the format the resampler works in, and its history holds
   std::vector<uint8_t> proto_x, phases_x;
+  ArsIo io = ArsIo ();           // how the caller's samples are stored (io.kind == ARS_IO_NONE: as fmt)
+  int width = 4;                 // bytes per sample in the caller's buffers
 };
 
 enum ArsFmt : int { ARS_F32 = 0, ARS_S16 = 1, ARS_S32 = 2, ARS_F64 = 3 };
+
+// Every GstAudioFormat (audio-format.c formats[], :249-418): packed width and step in bytes, depth, signedness, byte order,
+// float.  The step differs from the width only in the 20-bit _32 formats, whose pack / unpack functions are the 3-byte
+// ones (MAKE_PACK_UNPACK (s20_32le, 3, ...), audio-format.c:206-213).  Integer formats unpack to S32 and float formats to
+// F64 (their unpack_format); the quantize shift of an integer format is 32 - depth.
+static const struct ArsFormatInfo { int format, width, step, depth; bool is_signed, big, is_float; } kArsFormats[] = {
+  {B200_AUDIO_FORMAT_S8, 1, 1, 8, true, false, false},           {B200_AUDIO_FORMAT_U8, 1, 1, 8, false, false, false},
+  {B200_AUDIO_FORMAT_S16LE, 2, 2, 16, true, false, false},       {B200_AUDIO_FORMAT_S16BE, 2, 2, 16, true, true, false},
+  {B200_AUDIO_FORMAT_U16LE, 2, 2, 16, false, false, false},      {B200_AUDIO_FORMAT_U16BE, 2, 2, 16, false, true, false},
+  {B200_AUDIO_FORMAT_S24_32LE, 4, 4, 24, true, false, false},    {B200_AUDIO_FORMAT_S24_32BE, 4, 4, 24, true, true, false},
+  {B200_AUDIO_FORMAT_U24_32LE, 4, 4, 24, false, false, false},   {B200_AUDIO_FORMAT_U24_32BE, 4, 4, 24, false, true, false},
+  {B200_AUDIO_FORMAT_S32LE, 4, 4, 32, true, false, false},       {B200_AUDIO_FORMAT_S32BE, 4, 4, 32, true, true, false},
+  {B200_AUDIO_FORMAT_U32LE, 4, 4, 32, false, false, false},      {B200_AUDIO_FORMAT_U32BE, 4, 4, 32, false, true, false},
+  {B200_AUDIO_FORMAT_S24LE, 3, 3, 24, true, false, false},       {B200_AUDIO_FORMAT_S24BE, 3, 3, 24, true, true, false},
+  {B200_AUDIO_FORMAT_U24LE, 3, 3, 24, false, false, false},      {B200_AUDIO_FORMAT_U24BE, 3, 3, 24, false, true, false},
+  {B200_AUDIO_FORMAT_S20LE, 3, 3, 20, true, false, false},       {B200_AUDIO_FORMAT_S20BE, 3, 3, 20, true, true, false},
+  {B200_AUDIO_FORMAT_U20LE, 3, 3, 20, false, false, false},      {B200_AUDIO_FORMAT_U20BE, 3, 3, 20, false, true, false},
+  {B200_AUDIO_FORMAT_S18LE, 3, 3, 18, true, false, false},       {B200_AUDIO_FORMAT_S18BE, 3, 3, 18, true, true, false},
+  {B200_AUDIO_FORMAT_U18LE, 3, 3, 18, false, false, false},      {B200_AUDIO_FORMAT_U18BE, 3, 3, 18, false, true, false},
+  {B200_AUDIO_FORMAT_F32LE, 4, 4, 32, true, false, true},        {B200_AUDIO_FORMAT_F32BE, 4, 4, 32, true, true, true},
+  {B200_AUDIO_FORMAT_F64LE, 8, 8, 64, true, false, true},        {B200_AUDIO_FORMAT_F64BE, 8, 8, 64, true, true, true},
+  {B200_AUDIO_FORMAT_S20_32LE, 4, 3, 20, true, false, false},    {B200_AUDIO_FORMAT_S20_32BE, 4, 3, 20, true, true, false},
+  {B200_AUDIO_FORMAT_U20_32LE, 4, 3, 20, false, false, false},   {B200_AUDIO_FORMAT_U20_32BE, 4, 3, 20, false, true, false},
+};
 
 // convert_taps_gint16_c / _gint32_c (audio-resampler.c:217-258): round with a bias found by bisection so that
 // the integer taps sum to (1 << precision) - 1
@@ -160,8 +200,23 @@ static int build_ars_plan (const b200_ars_config & cfg, ArsPlan * p, int forced_
     case B200_AUDIO_FORMAT_S16LE: p->fmt = ARS_S16; p->bps = 2; break;
     case B200_AUDIO_FORMAT_S32LE: p->fmt = ARS_S32; p->bps = 4; break;
     case B200_AUDIO_FORMAT_F64LE: p->fmt = ARS_F64; p->bps = 8; break;
-    default: return B200_ERR_UNSUPPORTED;
+    default: {                   // unpacked to the format's unpack_format
+      const ArsFormatInfo *f = nullptr;
+      for (const ArsFormatInfo & e : kArsFormats) if (e.format == cfg.format) f = &e;
+      if (!f) return B200_ERR_UNSUPPORTED;
+      p->fmt = f->is_float ? ARS_F64 : ARS_S32;
+      p->bps = f->is_float ? 8 : 4;
+      p->io.kind = !f->is_float ? ARS_IO_INT : (f->width == 4 ? ARS_IO_F32 : ARS_IO_F64);
+      p->io.step = f->step;
+      p->io.big = f->big;
+      p->io.shift = f->is_float ? 0 : 32 - f->depth;
+      p->io.arith = f->is_signed && f->step == 4;
+      p->io.qshift = f->is_float ? 0 : 32 - f->depth;
+      p->io.sign = f->is_signed ? 0u : 0x80000000u;
+      p->width = f->width;
+    }
   }
+  if (p->io.kind == ARS_IO_NONE) p->width = p->bps;
   p->channels = cfg.channels;
   int a = cfg.in_rate, b = cfg.out_rate;
   while (b) { int t = a; a = b; b = t % b; }
@@ -1279,10 +1334,96 @@ __device__ __forceinline__ T ars_sample (const ArsLaunchX & L, long long f, int 
   return (T) 0;
 }
 
+// ---- packed samples: unpack, quantize, pack (audio-format.c MAKE_ORC_PACK_UNPACK / MAKE_PACK_UNPACK :116-217, the ORC
+// programs of gstaudiopack.orc, audio-quantize.c gst_audio_quantize_quantize_int_none_none :88-95)
+__device__ __forceinline__ unsigned long long ars_read_bytes (const ArsIo & io, const unsigned char *p)
+{
+  unsigned long long x = 0;
+  for (int b = 0; b < io.step; b++) x |= (unsigned long long) __ldg (p + b) << (8 * (io.big ? io.step - 1 - b : b));
+  return x;
+}
+__device__ __forceinline__ void ars_write_bytes (const ArsIo & io, unsigned char *p, unsigned long long x)
+{
+  for (int b = 0; b < io.step; b++) p[b] = (unsigned char) (x >> (8 * (io.big ? io.step - 1 - b : b)));
+}
+// the _trunc unpackers: the sample's bits moved to the top of 32 (bits shifted past bit 31 are lost), the sign bit flipped
+// for unsigned formats
+__device__ __forceinline__ int ars_unpack_int (const ArsIo & io, const unsigned char *p)
+{
+  return (int) (((unsigned) ars_read_bytes (io, p) << io.shift) ^ io.sign);
+}
+// bit casts and the double -> float narrowing (round to nearest), also in the emulated build
+#ifndef B200_CUDA_EMU
+__device__ __forceinline__ float ars_f32_of (unsigned b) { return __uint_as_float (b); }
+__device__ __forceinline__ unsigned ars_bits_f32 (float f) { return __float_as_uint (f); }
+__device__ __forceinline__ double ars_f64_of (unsigned long long b) { return __longlong_as_double ((long long) b); }
+__device__ __forceinline__ unsigned long long ars_bits_f64 (double d) { return (unsigned long long) __double_as_longlong (d); }
+__device__ __forceinline__ float ars_narrow (double d) { return __double2float_rn (d); }
+#else
+inline float ars_f32_of (unsigned b) { float f; memcpy (&f, &b, 4); return f; }
+inline unsigned ars_bits_f32 (float f) { unsigned b; memcpy (&b, &f, 4); return b; }
+inline double ars_f64_of (unsigned long long b) { double d; memcpy (&d, &b, 8); return d; }
+inline unsigned long long ars_bits_f64 (double d) { unsigned long long b; memcpy (&b, &d, 8); return b; }
+inline float ars_narrow (double d) { return (float) d; }
+#endif
+// ORC_DENORMAL: convfd / convdf flush denormals to a signed zero
+__device__ __forceinline__ unsigned ars_flush_f32 (unsigned b) { return (b & 0x7f800000u) ? b : (b & 0xff800000u); }
+__device__ __forceinline__ unsigned long long ars_flush_f64 (unsigned long long b)
+{
+  return (b & 0x7ff0000000000000ull) ? b : (b & 0xfff0000000000000ull);
+}
+__device__ __forceinline__ double ars_unpack_f64 (const ArsIo & io, const unsigned char *p)
+{
+  const unsigned long long x = ars_read_bytes (io, p);
+  if (io.kind == ARS_IO_F32) return (double) ars_f32_of (ars_flush_f32 ((unsigned) x));
+  return ars_f64_of (x);
+}
+// audio_orc_int_bias: saturating add of half a step, then the bits below the depth cleared; the pack's shift back down
+__device__ __forceinline__ void ars_pack_int (const ArsIo & io, unsigned char *p, int v)
+{
+  if (io.qshift) {
+    const long long t = (long long) v + (1LL << (io.qshift - 1));
+    v = (int) (t > 2147483647LL ? 2147483647LL : t) & ~((1 << io.qshift) - 1);
+  }
+  const unsigned u = (unsigned) v ^ io.sign;
+  ars_write_bytes (io, p, io.arith ? (unsigned) ((int) u >> io.shift) : u >> io.shift);
+}
+__device__ __forceinline__ void ars_pack_f64 (const ArsIo & io, unsigned char *p, double v)
+{
+  if (io.kind == ARS_IO_F32) {
+    const float f = ars_narrow (ars_f64_of (ars_flush_f64 (ars_bits_f64 (v))));
+    ars_write_bytes (io, p, ars_flush_f32 (ars_bits_f32 (f)));
+  } else
+    ars_write_bytes (io, p, ars_bits_f64 (v));
+}
 
-template <int FMT, bool LIN>
-__global__ void __launch_bounds__ (ARS_THREADS)
-ars_direct_kernel (const ArsLaunchX L)
+// How a kernel body reads a stream sample and writes an output sample.  ArsPlainIo: the caller's buffers hold the
+// resampler's own format.  ArsPackedIo: the caller's samples are unpacked on load and quantized and packed on store; the
+// history always holds the resampler's format.
+struct ArsPlainIo {
+  template <typename T> __device__ __forceinline__ T load (const ArsLaunchX & L, long long f, int c) const { return ars_sample<T> (L, f, c); }
+  template <typename T> __device__ __forceinline__ void store (const ArsLaunchX & L, size_t at, T v) const { ((T *) L.out)[at] = v; }
+};
+struct ArsPackedIo {
+  ArsIo io;
+  template <typename T> __device__ __forceinline__ T load (const ArsLaunchX & L, long long f, int c) const
+  {
+    if (f < L.hist_frames) return __ldg ((const T *) L.hist + f * L.channels + c);
+    if (!L.in) return (T) 0;
+    const unsigned char *p = (const unsigned char *) L.in + (size_t) ((f - L.hist_frames) * L.channels + c) * io.step;
+    return sizeof (T) == 8 ? (T) ars_unpack_f64 (io, p) : (T) ars_unpack_int (io, p);
+  }
+  template <typename T> __device__ __forceinline__ void store (const ArsLaunchX & L, size_t at, T v) const
+  {
+    unsigned char *p = (unsigned char *) L.out + at * io.step;
+    if (sizeof (T) == 8) ars_pack_f64 (io, p, (double) v);
+    else ars_pack_int (io, p, (int) v);
+  }
+};
+
+
+template <int FMT, bool LIN, class IO>
+__device__ __forceinline__ void ars_direct_body (const ArsLaunchX & L, const IO & io)
 {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const long long o = (long long) blockIdx.x * (ARS_THREADS / 32) + warp;
@@ -1301,8 +1442,8 @@ ars_direct_kernel (const ArsLaunchX L)
     const short *tab = (const short *) L.table + row0;
     if (L.full) {                 // inner_product_gint16_full_1_sse2
       unsigned sum = 0;
-      for (int i = 0; i < n; i++) sum += (unsigned) ((int) ars_sample<short> (L, idx + i, c) * (int) __ldg (tab + i));
-      ((short *) L.out)[(size_t) o * L.channels + c] = (short) ars_round_s16 (sum);
+      for (int i = 0; i < n; i++) sum += (unsigned) ((int) io.template load<short> (L, idx + i, c) * (int) __ldg (tab + i));
+      io.template store<short> (L, (size_t) o * L.channels + c, (short) ars_round_s16 (sum));
     } else if (LIN) {             // inner_product_gint16_linear_1_sse2 (audio-resampler-x86-sse2.c:57-108): 32-bit lane l
       unsigned s[2][4];           // sums the tap pairs (2l, 2l+1) of every eight; each LANE is shifted and multiplied
 #pragma unroll
@@ -1312,7 +1453,7 @@ ars_direct_kernel (const ArsLaunchX L)
       for (int i = 0; i < n; i += 8)
 #pragma unroll
         for (int j = 0; j < 8; j++) {
-          const int x = ars_sample<short> (L, idx + i + j, c);
+          const int x = io.template load<short> (L, idx + i + j, c);
           s[0][j >> 1] += (unsigned) (x * (int) __ldg (tab + i + j));
           s[1][j >> 1] += (unsigned) (x * (int) __ldg (tab + n + i + j));
         }
@@ -1321,11 +1462,11 @@ ars_direct_kernel (const ArsLaunchX L)
 #pragma unroll
       for (int l = 0; l < 4; l++)
         acc += (unsigned) ((int) (short) ((int) s[0][l] >> 15) * x) + (unsigned) ((int) (short) ((int) s[1][l] >> 15) * y);
-      ((short *) L.out)[(size_t) o * L.channels + c] = (short) ars_round_s16 (acc);
+      io.template store<short> (L, (size_t) o * L.channels + c, (short) ars_round_s16 (acc));
     } else {                      // inner_product_gint16_cubic_1_sse2
       unsigned s0 = 0, s1 = 0, s2 = 0, s3 = 0;
       for (int i = 0; i < n; i++) {
-        const int x = ars_sample<short> (L, idx + i, c);
+        const int x = io.template load<short> (L, idx + i, c);
         s0 += (unsigned) (x * (int) __ldg (tab + i));
         s1 += (unsigned) (x * (int) __ldg (tab + n + i));
         s2 += (unsigned) (x * (int) __ldg (tab + 2 * n + i));
@@ -1335,21 +1476,21 @@ ars_direct_kernel (const ArsLaunchX L)
       cubic_coeff_s16 (frac, L.out_step, ic);
       const unsigned acc = (unsigned) ((int) (short) ((int) s0 >> 15) * ic[0]) + (unsigned) ((int) (short) ((int) s1 >> 15) * ic[1]) +
           (unsigned) ((int) (short) ((int) s2 >> 15) * ic[2]) + (unsigned) ((int) (short) ((int) s3 >> 15) * ic[3]);
-      ((short *) L.out)[(size_t) o * L.channels + c] = (short) ars_round_s16 (acc);
+      io.template store<short> (L, (size_t) o * L.channels + c, (short) ars_round_s16 (acc));
     }
   } else if (FMT == ARS_S32) {
     const int *tab = (const int *) L.table + row0;
     if (L.full) {                 // inner_product_gint32_full_1_sse41
       unsigned long long sum = 0;
-      for (int i = 0; i < n; i++) sum += (unsigned long long) ((long long) ars_sample<int> (L, idx + i, c) * __ldg (tab + i));
-      ((int *) L.out)[(size_t) o * L.channels + c] = ars_round_s32 (sum);
+      for (int i = 0; i < n; i++) sum += (unsigned long long) ((long long) io.template load<int> (L, idx + i, c) * __ldg (tab + i));
+      io.template store<int> (L, (size_t) o * L.channels + c, ars_round_s32 (sum));
     } else {                      // inner_product_gint32_cubic_1_sse41: each 64-bit LANE (even / odd taps) is
       unsigned long long s[4][2]; // shifted and multiplied before the lanes are added; _linear_1_sse41 (:70-112) is the same
       constexpr int ROWS = LIN ? 2 : 4;   // arithmetic over two rows
 #pragma unroll
       for (int k = 0; k < 4; k++) s[k][0] = s[k][1] = 0;
       for (int i = 0; i < n; i += 2) {
-        const long long x0 = ars_sample<int> (L, idx + i, c), x1 = ars_sample<int> (L, idx + i + 1, c);
+        const long long x0 = io.template load<int> (L, idx + i, c), x1 = io.template load<int> (L, idx + i + 1, c);
 #pragma unroll
         for (int k = 0; k < ROWS; k++) {
           s[k][0] += (unsigned long long) (x0 * __ldg (tab + k * n + i));
@@ -1368,21 +1509,21 @@ ars_direct_kernel (const ArsLaunchX L)
 #pragma unroll
         for (int l = 0; l < 2; l++)
           acc += (unsigned long long) ((long long) (int) (unsigned) (s[k][l] >> 31) * (long long) ic[k]);
-      ((int *) L.out)[(size_t) o * L.channels + c] = ars_round_s32 (acc);
+      io.template store<int> (L, (size_t) o * L.channels + c, ars_round_s32 (acc));
     }
   } else {
     const double *tab = (const double *) L.table + row0;
     if (L.full) {                 // inner_product_gdouble_full_1_sse2
       double s0 = 0.0, s1 = 0.0;
       for (int i = 0; i < n; i += 2) {
-        s0 = __dadd_rn (s0, __dmul_rn (ars_sample<double> (L, idx + i, c), __ldg (tab + i)));
-        s1 = __dadd_rn (s1, __dmul_rn (ars_sample<double> (L, idx + i + 1, c), __ldg (tab + i + 1)));
+        s0 = __dadd_rn (s0, __dmul_rn (io.template load<double> (L, idx + i, c), __ldg (tab + i)));
+        s1 = __dadd_rn (s1, __dmul_rn (io.template load<double> (L, idx + i + 1, c), __ldg (tab + i + 1)));
       }
-      ((double *) L.out)[(size_t) o * L.channels + c] = __dadd_rn (s0, s1);
+      io.template store<double> (L, (size_t) o * L.channels + c, __dadd_rn (s0, s1));
     } else if (LIN) {             // inner_product_gdouble_linear_1_sse2 (audio-resampler-x86-sse2.c:195-220)
       double s[2][2] = {{0.0, 0.0}, {0.0, 0.0}};
       for (int i = 0; i < n; i += 2) {
-        const double x0 = ars_sample<double> (L, idx + i, c), x1 = ars_sample<double> (L, idx + i + 1, c);
+        const double x0 = io.template load<double> (L, idx + i, c), x1 = io.template load<double> (L, idx + i + 1, c);
 #pragma unroll
         for (int k = 0; k < 2; k++) {
           s[k][0] = __dadd_rn (s[k][0], __dmul_rn (x0, __ldg (tab + k * n + i)));
@@ -1392,13 +1533,13 @@ ars_direct_kernel (const ArsLaunchX L)
       const double x = __ddiv_rn ((double) frac, (double) L.out_step);      // make_coeff_gdouble_linear: ic[0]
       const double l0 = __dadd_rn (__dmul_rn (__dsub_rn (s[0][0], s[1][0]), x), s[1][0]);
       const double l1 = __dadd_rn (__dmul_rn (__dsub_rn (s[0][1], s[1][1]), x), s[1][1]);
-      ((double *) L.out)[(size_t) o * L.channels + c] = __dadd_rn (l0, l1);
+      io.template store<double> (L, (size_t) o * L.channels + c, __dadd_rn (l0, l1));
     } else {                      // inner_product_gdouble_cubic_1_sse2
       double s[4][2];
 #pragma unroll
       for (int k = 0; k < 4; k++) s[k][0] = s[k][1] = 0.0;
       for (int i = 0; i < n; i += 2) {
-        const double x0 = ars_sample<double> (L, idx + i, c), x1 = ars_sample<double> (L, idx + i + 1, c);
+        const double x0 = io.template load<double> (L, idx + i, c), x1 = io.template load<double> (L, idx + i + 1, c);
 #pragma unroll
         for (int k = 0; k < 4; k++) {
           s[k][0] = __dadd_rn (s[k][0], __dmul_rn (x0, __ldg (tab + k * n + i)));
@@ -1417,9 +1558,30 @@ ars_direct_kernel (const ArsLaunchX L)
       for (int j = 0; j < 2; j++)
         l[j] = __dadd_rn (__dadd_rn (__dmul_rn (s[0][j], ic0), __dmul_rn (s[1][j], ic1)),
             __dadd_rn (__dmul_rn (s[2][j], ic2), __dmul_rn (s[3][j], ic3)));
-      ((double *) L.out)[(size_t) o * L.channels + c] = __dadd_rn (l[0], l[1]);
+      io.template store<double> (L, (size_t) o * L.channels + c, __dadd_rn (l[0], l[1]));
     }
   }
+}
+
+// The resampler in S32 / F64 (its history) over the caller's own samples (ArsLaunchX) or over packed ones (ArsLaunchP:
+// unpacked on load, quantized and packed on store; the launch's descriptor is uniform across the grid)
+struct ArsLaunchP {
+  ArsLaunchX x;
+  ArsIo io;
+};
+
+template <int FMT, bool LIN>
+__global__ void __launch_bounds__ (ARS_THREADS)
+ars_direct_kernel (const ArsLaunchX L)
+{
+  ars_direct_body<FMT, LIN> (L, ArsPlainIo ());
+}
+
+template <int FMT, bool LIN>
+__global__ void __launch_bounds__ (ARS_THREADS)
+ars_direct_kernel_packed (const ArsLaunchP L)
+{
+  ars_direct_body<FMT, LIN> (L.x, ArsPackedIo {L.io});
 }
 
 // resample-method nearest / linear / cubic: a handful of taps per output (2, 4, or those scaled by the decimation
@@ -1428,9 +1590,8 @@ ars_direct_kernel (const ArsLaunchX L)
 // stop at n_taps: F32 four lanes by tap index mod 4 and (l0 + l2) + (l1 + l3) (inner_product_gfloat_full_1_sse), F64 two
 // lanes by parity, the integer sums exact.  Nearest copies the first sample of the window
 // (inner_product_<type>_nearest_1_c :602-612).  Warp = one output frame x 32 channels.
-template <int FMT>
-__global__ void __launch_bounds__ (ARS_THREADS)
-ars_small_kernel (const ArsLaunchX L, int nearest)
+template <int FMT, class IO>
+__device__ __forceinline__ void ars_small_body (const ArsLaunchX & L, int nearest, const IO & io)
 {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const long long o = (long long) blockIdx.x * (ARS_THREADS / 32) + warp;
@@ -1442,36 +1603,50 @@ ars_small_kernel (const ArsLaunchX L, int nearest)
   const int phase = (int) (t0 % L.out_step), n = L.n_taps;
   const size_t at = (size_t) o * L.channels + c, row0 = (size_t) phase * n;
   if (FMT == ARS_S16) {
-    if (nearest) { ((short *) L.out)[at] = ars_sample<short> (L, idx, c); return; }
+    if (nearest) { io.template store<short> (L, at, io.template load<short> (L, idx, c)); return; }
     const short *tab = (const short *) L.table + row0;
     unsigned sum = 0;
-    for (int i = 0; i < n; i++) sum += (unsigned) ((int) ars_sample<short> (L, idx + i, c) * (int) __ldg (tab + i));
-    ((short *) L.out)[at] = (short) ars_round_s16 (sum);
+    for (int i = 0; i < n; i++) sum += (unsigned) ((int) io.template load<short> (L, idx + i, c) * (int) __ldg (tab + i));
+    io.template store<short> (L, at, (short) ars_round_s16 (sum));
   } else if (FMT == ARS_S32) {
-    if (nearest) { ((int *) L.out)[at] = ars_sample<int> (L, idx, c); return; }
+    if (nearest) { io.template store<int> (L, at, io.template load<int> (L, idx, c)); return; }
     const int *tab = (const int *) L.table + row0;
     unsigned long long sum = 0;
-    for (int i = 0; i < n; i++) sum += (unsigned long long) ((long long) ars_sample<int> (L, idx + i, c) * __ldg (tab + i));
-    ((int *) L.out)[at] = ars_round_s32 (sum);
+    for (int i = 0; i < n; i++) sum += (unsigned long long) ((long long) io.template load<int> (L, idx + i, c) * __ldg (tab + i));
+    io.template store<int> (L, at, ars_round_s32 (sum));
   } else if (FMT == ARS_F64) {
-    if (nearest) { ((double *) L.out)[at] = ars_sample<double> (L, idx, c); return; }
+    if (nearest) { io.template store<double> (L, at, io.template load<double> (L, idx, c)); return; }
     const double *tab = (const double *) L.table + row0;
     double s0 = 0.0, s1 = 0.0;
     for (int i = 0; i < n; i += 2) {
-      s0 = __dadd_rn (s0, __dmul_rn (ars_sample<double> (L, idx + i, c), __ldg (tab + i)));
-      if (i + 1 < n) s1 = __dadd_rn (s1, __dmul_rn (ars_sample<double> (L, idx + i + 1, c), __ldg (tab + i + 1)));
+      s0 = __dadd_rn (s0, __dmul_rn (io.template load<double> (L, idx + i, c), __ldg (tab + i)));
+      if (i + 1 < n) s1 = __dadd_rn (s1, __dmul_rn (io.template load<double> (L, idx + i + 1, c), __ldg (tab + i + 1)));
     }
-    ((double *) L.out)[at] = __dadd_rn (s0, s1);
+    io.template store<double> (L, at, __dadd_rn (s0, s1));
   } else {
-    if (nearest) { ((float *) L.out)[at] = ars_sample<float> (L, idx, c); return; }
+    if (nearest) { io.template store<float> (L, at, io.template load<float> (L, idx, c)); return; }
     const float *tab = (const float *) L.table + row0;
     float s[4] = {0.f, 0.f, 0.f, 0.f};
     for (int i = 0; i < n; i += 4)
 #pragma unroll
       for (int l = 0; l < 4; l++)
-        if (i + l < n) s[l] = __fadd_rn (s[l], __fmul_rn (ars_sample<float> (L, idx + i + l, c), __ldg (tab + i + l)));
-    ((float *) L.out)[at] = ars_lane_sum (s);
+        if (i + l < n) s[l] = __fadd_rn (s[l], __fmul_rn (io.template load<float> (L, idx + i + l, c), __ldg (tab + i + l)));
+    io.template store<float> (L, at, ars_lane_sum (s));
   }
+}
+
+template <int FMT>
+__global__ void __launch_bounds__ (ARS_THREADS)
+ars_small_kernel (const ArsLaunchX L, int nearest)
+{
+  ars_small_body<FMT> (L, nearest, ArsPlainIo ());
+}
+
+template <int FMT>
+__global__ void __launch_bounds__ (ARS_THREADS)
+ars_small_kernel_packed (const ArsLaunchP L, int nearest)
+{
+  ars_small_body<FMT> (L.x, nearest, ArsPackedIo {L.io});
 }
 
 // new history = frames [first, first+keep) of the (old history ++ input) stream, any sample width
@@ -1500,6 +1675,24 @@ __global__ void ars_history_kernel (float *dst, const float *hist, const float *
     int channels)
 {
   ars_history_copy (dst, hist, in, hist_frames, first, keep, channels);
+}
+// the same for packed input: the kept input samples are unpacked into the history, which holds T (int: S32, double: F64)
+template <typename T>
+__global__ void ars_history_kernel_packed (T *dst, const T *hist, const unsigned char *in, ArsIo io, long long hist_frames,
+    long long first, long long keep, int channels)
+{
+  const long long n = keep * channels;
+  for (long long i = blockIdx.x * (long long) blockDim.x + threadIdx.x; i < n; i += (long long) gridDim.x * blockDim.x) {
+    const long long f = first + i / channels;
+    const int c = (int) (i % channels);
+    T v = 0;
+    if (f < hist_frames) v = hist[f * channels + c];
+    else if (in) {
+      const unsigned char *p = in + (size_t) ((f - hist_frames) * channels + c) * io.step;
+      v = sizeof (T) == 8 ? (T) ars_unpack_f64 (io, p) : (T) ars_unpack_int (io, p);
+    }
+    dst[i] = v;
+  }
 }
 
 }  // namespace b200
@@ -1903,6 +2096,17 @@ int b200_ars_process (b200_ars * h, const void *in_v, size_t in_frames, void *ou
     auto tiles = [&] { return dim3 ((unsigned) ((out_frames + r.no - 1) / r.no), (unsigned) ((p.channels + r.cb - 1) / r.cb)); };
     const int nearest = p.small == B200_ARS_METHOD_NEAREST || p.copy;
     const bool lin = p.linear && !p.full;
+    // packed samples reach only the S32 / F64 routes: the small and direct kernels
+    const ArsLaunchP P = {X, p.io};
+    if (p.io.kind != ARS_IO_NONE && r.kern == ARS_K_SMALL) {
+      if (p.fmt == ARS_S32) ars_small_kernel_packed<ARS_S32> <<<warps, ARS_THREADS, 0, stream>>> (P, nearest);
+      else ars_small_kernel_packed<ARS_F64> <<<warps, ARS_THREADS, 0, stream>>> (P, nearest);
+    } else if (p.io.kind != ARS_IO_NONE) {
+      if (p.fmt == ARS_S32 && lin) ars_direct_kernel_packed<ARS_S32, true> <<<warps, ARS_THREADS, 0, stream>>> (P);
+      else if (p.fmt == ARS_S32) ars_direct_kernel_packed<ARS_S32, false> <<<warps, ARS_THREADS, 0, stream>>> (P);
+      else if (lin) ars_direct_kernel_packed<ARS_F64, true> <<<warps, ARS_THREADS, 0, stream>>> (P);
+      else ars_direct_kernel_packed<ARS_F64, false> <<<warps, ARS_THREADS, 0, stream>>> (P);
+    } else
     switch (r.kern) {
       case ARS_K_SMALL:
         if (p.fmt == ARS_S16) ars_small_kernel<ARS_S16> <<<warps, ARS_THREADS, 0, stream>>> (X, nearest);
@@ -1944,7 +2148,7 @@ int b200_ars_process (b200_ars * h, const void *in_v, size_t in_frames, void *ou
         if (h->knobs.grid) grid = std::min (grid, h->knobs.grid);
         ArsTensorMap tm = ArsTensorMap ();
         const int use_tm = r.kern != ARS_K_PIPE_V1 && !h->knobs.no_tensormap &&
-            ars_encode_window_map (&tm, in_v, (unsigned long long) in_frames, p.channels, ARS_PIPE_CB, T.win, p.bps);
+            ars_encode_window_map (&tm, in_v, (unsigned long long) in_frames, p.channels, ARS_PIPE_CB, T.win, p.width);
         if (r.kern == ARS_K_PIPE) ars_pipe_kernel <<<grid, ARS_PIPE_THREADS, r.smem, stream>>> (L, T, n_fb, n_cb, tm, use_tm);
         else if (r.kern == ARS_K_PIPE_S16) ars_pipe_kernel_s16 <<<grid, ARS_PIPE_THREADS, r.smem, stream>>> (L, T, n_fb, n_cb, tm, use_tm);
         else ars_pipe_kernel_v1 <<<grid, ARS_PIPE_THREADS, r.smem, stream>>> (L, T, n_fb, n_cb);
@@ -1981,7 +2185,15 @@ int b200_ars_process (b200_ars * h, const void *in_v, size_t in_frames, void *ou
     const long long n = (long long) count * p.channels;
     const int blocks = (int) ((n + 255) / 256 > 1184 ? 1184 : (n + 255) / 256);
     const size_t off = dst_frame * p.channels;
-    if (p.bps == 2)
+    if (p.io.kind != ARS_IO_NONE && p.bps == 8)
+      ars_history_kernel_packed<double> <<<blocks, 256, 0, stream>>> ((double *) h->d_hist[nxt] + off,
+          (const double *) h->d_hist[h->cur], (const unsigned char *) in_v, p.io, (long long) hist, from, (long long) count,
+          p.channels);
+    else if (p.io.kind != ARS_IO_NONE)
+      ars_history_kernel_packed<int> <<<blocks, 256, 0, stream>>> ((int *) h->d_hist[nxt] + off,
+          (const int *) h->d_hist[h->cur], (const unsigned char *) in_v, p.io, (long long) hist, from, (long long) count,
+          p.channels);
+    else if (p.bps == 2)
       ars_history_kernel_x<unsigned short> <<<blocks, 256, 0, stream>>> ((unsigned short *) h->d_hist[nxt] + off,
           (const unsigned short *) h->d_hist[h->cur], (const unsigned short *) in_v, (long long) hist, from,
           (long long) count, p.channels);
@@ -2026,7 +2238,7 @@ int b200_ars_process_host_submit (b200_ars * h, const void *in_host, size_t in_f
   DeviceGuard g (h->device);
   if (!g.ok) return B200_ERR_CUDA;
   B200_CUDA_TRY (h->ring.setup ());
-  const size_t bpf = (size_t) h->plan.channels * h->plan.bps;
+  const size_t bpf = (size_t) h->plan.channels * h->plan.width;     // the caller's samples
   const size_t in_bytes = in_host ? in_frames * bpf : 0;
   const size_t want = b200_ars_get_out_frames (h, in_frames);
   if (want > out_capacity_frames) return B200_ERR_INVALID_ARG;
@@ -2039,7 +2251,9 @@ int b200_ars_process_host_submit (b200_ars * h, const void *in_host, size_t in_f
   int st = b200_ars_process (h, in_host ? r.in () : nullptr, in_frames, r.out (), want, &got, r.run_stream ());
   if (st != B200_OK) return st;
   B200_CUDA_TRY (r.run_done ());
-  if (got) B200_CUDA_TRY (r.download (out_host, r.out (), got * bpf));
+  // the bytes the kernels wrote: the 20-bit _32 formats leave the last quarter of the caller's frames as it was
+  const size_t written = (size_t) h->plan.channels * (h->plan.io.kind != ARS_IO_NONE ? h->plan.io.step : h->plan.width);
+  if (got) B200_CUDA_TRY (r.download (out_host, r.out (), got * written));
   B200_CUDA_TRY (r.finish ());
   if (out_frames) *out_frames = got;
   return B200_OK;

@@ -300,14 +300,26 @@ int b200_comp_blend_convert (b200_comp * h, void *dst, const b200_video_info * d
 
 /* ------------------------------------------------------------------ audio resampler */
 typedef struct b200_ars b200_ars;
-/* GstAudioFormat values (gst-libs/gst/audio/audio-format.h:97-140) of the sample formats audioresample hands to
- * its resampler unconverted (audio-converter.c:700-727), native (little) endian */
-enum { B200_AUDIO_FORMAT_S16LE = 4, B200_AUDIO_FORMAT_S32LE = 12, B200_AUDIO_FORMAT_F32LE = 28,
-  B200_AUDIO_FORMAT_F64LE = 30 };
+/* GstAudioFormat values (gst-libs/gst/audio/audio-format.h:97-140).  S16LE, S32LE, F32LE and F64LE are resampled as they
+ * are (audio-converter.c:700-727); every other format is unpacked to S32 (integer formats) or F64 (F32BE, F64BE) on
+ * load, resampled in that format, and quantized and packed back on store, as audioresample's converter does
+ * (converter_generic, audio-converter.c:1281-1310). */
+enum { B200_AUDIO_FORMAT_S8 = 2, B200_AUDIO_FORMAT_U8 = 3, B200_AUDIO_FORMAT_S16LE = 4, B200_AUDIO_FORMAT_S16BE = 5,
+  B200_AUDIO_FORMAT_U16LE = 6, B200_AUDIO_FORMAT_U16BE = 7, B200_AUDIO_FORMAT_S24_32LE = 8, B200_AUDIO_FORMAT_S24_32BE = 9,
+  B200_AUDIO_FORMAT_U24_32LE = 10, B200_AUDIO_FORMAT_U24_32BE = 11, B200_AUDIO_FORMAT_S32LE = 12, B200_AUDIO_FORMAT_S32BE = 13,
+  B200_AUDIO_FORMAT_U32LE = 14, B200_AUDIO_FORMAT_U32BE = 15, B200_AUDIO_FORMAT_S24LE = 16, B200_AUDIO_FORMAT_S24BE = 17,
+  B200_AUDIO_FORMAT_U24LE = 18, B200_AUDIO_FORMAT_U24BE = 19, B200_AUDIO_FORMAT_S20LE = 20, B200_AUDIO_FORMAT_S20BE = 21,
+  B200_AUDIO_FORMAT_U20LE = 22, B200_AUDIO_FORMAT_U20BE = 23, B200_AUDIO_FORMAT_S18LE = 24, B200_AUDIO_FORMAT_S18BE = 25,
+  B200_AUDIO_FORMAT_U18LE = 26, B200_AUDIO_FORMAT_U18BE = 27, B200_AUDIO_FORMAT_F32LE = 28, B200_AUDIO_FORMAT_F32BE = 29,
+  B200_AUDIO_FORMAT_F64LE = 30, B200_AUDIO_FORMAT_F64BE = 31, B200_AUDIO_FORMAT_S20_32LE = 32, B200_AUDIO_FORMAT_S20_32BE = 33,
+  B200_AUDIO_FORMAT_U20_32LE = 34, B200_AUDIO_FORMAT_U20_32BE = 35 };
 typedef struct {
   int32_t in_rate, out_rate, channels;
   int32_t quality;               /* 0..10, element default 4 (gstaudioresample.c:68) */
-  int32_t format;                /* B200_AUDIO_FORMAT_*; 0 = F32LE */
+  /* B200_AUDIO_FORMAT_*; 0 = F32LE.  Buffers hold interleaved samples of this format at its packed width (1, 2, 3, 4
+   * or 8 bytes; the 20-bit _32 formats are 4 bytes wide but, as in the reference, their samples lie 3 bytes apart
+   * and the last quarter of an output buffer is left as it was). */
+  int32_t format;
   /* the element's resample-method / sinc-filter-mode / sinc-filter-interpolation properties (gstaudioresample.c:160-186).
    * 0 = the element default in each; other values are the reference's enum value + 1 so that a zeroed config is the
    * default configuration: */
@@ -334,7 +346,8 @@ int b200_ars_update (b200_ars * h, int in_rate, int out_rate);
 size_t b200_ars_get_out_frames (b200_ars * h, size_t in_frames);
 size_t b200_ars_get_in_frames (b200_ars * h, size_t out_frames);
 size_t b200_ars_get_max_latency (b200_ars * h);
-/* Interleaved device buffers of the configured sample format.  in == NULL feeds silence (drain).
+/* Interleaved device buffers of the configured sample format at its packed width; the formats that are unpacked may
+ * start at any byte.  in == NULL feeds silence (drain).
  * Consumes all in_frames, writes b200_ars_get_out_frames() frames, asynchronous on cuda_stream. */
 int b200_ars_process (b200_ars * h, const void *in, size_t in_frames, void *out,
     size_t out_capacity_frames, size_t * out_frames, void *cuda_stream);
