@@ -159,7 +159,8 @@ class Setup:
         self.convs, self.frames, self.keep = {}, [], []
         for k, p in enumerate(case["pads"]):
             w, h, xo, yo = output_size(p)
-            a = random_frame(lib, p["in_fmt"], p["iw"], p["ih"], p["seed"])
+            # a case may bring its own content per pad (comp_fused_cases: worst cases of the pad's conversion)
+            a = case["content"](p) if "content" in case else random_frame(lib, p["in_fmt"], p["iw"], p["ih"], p["seed"])
             self.frames.append((a, w, h))
             ii = info(lib, p["in_fmt"], p["iw"], p["ih"], p["odd"])
             tight = unpack(p["in_fmt"], a, info(lib, p["in_fmt"], p["iw"], p["ih"]))
@@ -173,7 +174,7 @@ class Setup:
                     ci.color_matrix, ci.color_range, ci.chroma_site = self.di.color_matrix, self.di.color_range, self.di.chroma_site
                     cfg = _lib.VcsConfigC()
                     lib.b200_vcs_config_init(C.byref(cfg))
-                    cfg.method = MITCHELL
+                    cfg.method = case.get("method", MITCHELL)
                     hv = C.c_void_p()
                     assert lib.b200_vcs_create(C.byref(ii), C.byref(ci), C.byref(cfg), 0, C.byref(hv)) == 0, key
                     self.convs[key] = hv
@@ -228,7 +229,7 @@ class Setup:
         for k, p in enumerate(self.case["pads"]):
             a, w, h = self.frames[k]
             if self.pads[k].conv:
-                a = ob.oracle_vcs_convert(ob.vcs_desc(p["iw"], p["ih"], w, h, MITCHELL, in_fmt=FMT[p["in_fmt"]],
+                a = ob.oracle_vcs_convert(ob.vcs_desc(p["iw"], p["ih"], w, h, self.case.get("method", MITCHELL), in_fmt=FMT[p["in_fmt"]],
                                                       out_fmt=FMT[out]), a)
             keep.append(a)
             opads[k].data, opads[k].width, opads[k].height = a.ctypes.data, w, h

@@ -9,7 +9,7 @@ cd "$(dirname "$0")/.."
 AS=$(g++ -print-file-name=libasan.so)
 LOG=$(mktemp -d)/asan
 B200_EMU_ASAN=1 LD_PRELOAD=$AS ASAN_OPTIONS="detect_leaks=0:halt_on_error=0:log_path=$LOG" \
-  python -m pytest tests/test_emu_kernels.py tests/test_emu_batch.py tests/test_emu_worstcase.py tests/test_ars_packed_formats.py tests/test_comp_convert.py tests/test_host_staging.py -q -p no:cacheprovider ${1:+-k "$1"} | tail -3
+  python -m pytest tests/test_emu_kernels.py tests/test_emu_batch.py tests/test_emu_worstcase.py tests/test_ars_packed_formats.py tests/test_comp_convert.py tests/test_comp_domain.py tests/test_comp_fused.py tests/test_host_staging.py -q -p no:cacheprovider ${1:+-k "$1"} | tail -3
 n=$(cat "$LOG".* 2>/dev/null | grep -c "ERROR: AddressSanitizer")
 echo "memcheck: $n reports"
 cat "$LOG".* 2>/dev/null | grep -A3 "ERROR: AddressSanitizer" | grep "#0\|#1" | sort | uniq -c | sort -rn | head -10

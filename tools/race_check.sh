@@ -10,7 +10,7 @@ cd "$(dirname "$0")/.."
 TS=$(g++ -print-file-name=libtsan.so)
 LOG=$(mktemp -d)/tsan
 B200_EMU_TSAN=1 LD_PRELOAD=$TS TSAN_OPTIONS="halt_on_error=0 report_signal_unsafe=0 log_path=$LOG" \
-  python -m pytest tests/test_emu_kernels.py tests/test_emu_batch.py tests/test_emu_worstcase.py tests/test_ars_packed_formats.py tests/test_comp_convert.py -q -p no:cacheprovider ${1:+-k "$1"} | tail -3
+  python -m pytest tests/test_emu_kernels.py tests/test_emu_batch.py tests/test_emu_worstcase.py tests/test_ars_packed_formats.py tests/test_comp_convert.py tests/test_comp_domain.py tests/test_comp_fused.py -q -p no:cacheprovider ${1:+-k "$1"} | tail -3
 n=$(cat "$LOG".* 2>/dev/null | grep -c "WARNING: ThreadSanitizer")
 echo "race_check: $n reports"
 cat "$LOG".* 2>/dev/null | grep -A3 "WARNING: ThreadSanitizer: data race" | grep "#0" | sort | uniq -c | sort -rn | head -10
