@@ -289,10 +289,8 @@ inline L2mmaTables build_l2mma_tables (const VcsPlan & p)
   if ((p.in.stride[0] & 7) || (p.in.stride[1] & 7) || (p.in.offset[0] & 7) || (p.in.offset[1] & 7)) return t;
   if ((p.in.width & 7) || (p.in.height & 1) || p.in.width < 8) return t;
   if ((p.out.stride[0] & 3) || (p.out.offset[0] & 3)) return t;
-  for (int y = 0; y < p.in.height; y++)       // every line consumed in order: standard pairing
-    if (p.chroma_mode[y] != (y == 0 ? 0 : ((y & 1) ? 1 : 2))) return t;
-  for (int16_t s : p.h.sum) if (s < 64 || s > 128) return t;      // alpha stays 255 through both passes
-  for (int16_t s : p.v.sum) if (s < 64 || s > 128) return t;
+  if (!standard_pairing (p)) return t;
+  if (!alpha_stays_opaque (p.h) || !alpha_stays_opaque (p.v)) return t;     // alpha stays 255 through both passes
   if (!pack_axis_l2mma (p.h, 8, true, &t.bh, &t.h4)) return t;     // staged columns start 8 pixels left of the tile
   if (!pack_axis_l2mma (p.v, 3, false, &t.bv, &t.v4)) return t;    // staged lines start at 2*oy0 - 3
   t.ok = true;

@@ -387,13 +387,10 @@ inline Lanczos2Tables build_lanczos2_tables (const VcsPlan & p)
     for (int k = 1; k <= 2; k++) if ((p.in.stride[k] & 3) || (p.in.offset[k] & 3) || p.in.stride[k] < (p.in.width >> 1)) return t;
   } else if ((p.in.stride[0] & 7) || (p.in.stride[1] & 7) || (p.in.offset[0] & 7) || (p.in.offset[1] & 7)) return t;
   if ((p.in.width & 7) || (p.in.height & 1)) return t;
-  for (int y = 0; y < p.in.height; y++)       // every line consumed in order: standard pairing
-    if (p.chroma_mode[y] != (y == 0 ? 0 : ((y & 1) ? 1 : 2))) return t;
+  if (!standard_pairing (p)) return t;
   if (!pack_axis_lanczos2 (p.h, 4, &t.htab)) return t;
   if (!pack_axis_lanczos2 (p.v, 3, &t.vtab)) return t;
-  t.alpha_opaque = true;
-  for (int16_t s : p.h.sum) if (s < 64 || s > 128) t.alpha_opaque = false;
-  for (int16_t s : p.v.sum) if (s < 64 || s > 128) t.alpha_opaque = false;
+  t.alpha_opaque = alpha_stays_opaque (p.h) && alpha_stays_opaque (p.v);
   t.ok = true;
   // X4 tables: usable when every column group OUTSIDE the kernel's edge tiles (the first tile column and the tiles that
   // reach the right border: x0 == 0 || x0 + TW + 4 >= ow, TW = 120) fits; row groups are flagged one by one

@@ -340,8 +340,7 @@ inline ntap_kernel_fn ntap_kernel_pick (const VcsPlan & p)
 template <int HM, int VM>
 inline ntap_kernel_fn ntap_kernel_pick_ntw (const VcsPlan & p)
 {
-  int ntw = HM == 3 && VM == 3 ? (p.ntw_h == p.ntw_v ? p.ntw_h : 0) : (HM == 3 ? p.ntw_h : p.ntw_v);
-  switch (ntw) {
+  switch (common_tap_words (HM, VM, p.ntw_h, p.ntw_v)) {
     case 1: return ntap_kernel_pick<HM, VM, 1> (p);
     case 2: return ntap_kernel_pick<HM, VM, 2> (p);
     case 3: return ntap_kernel_pick<HM, VM, 3> (p);

@@ -324,19 +324,11 @@ void chroma_pairing (VcsPlan * p)
 
 void tile_geometry (VcsPlan * p)
 {
-  const int ow = p->out.width, oh = p->out.height;
+  const int ow = p->out.width;
   int tw = ow >= 64 ? 64 : (ow >= 32 ? 32 : 16), th = 16;
   const int budget = 200 * 1024;
   for (;;) {
-    int max_rows = 0, max_cols = 0;
-    for (int y0 = 0; y0 < oh; y0 += th) {
-      int y1 = std::min (y0 + th, oh) - 1;
-      max_rows = std::max (max_rows, (int) (p->v.offset[y1] + p->v.span - p->v.offset[y0]));
-    }
-    for (int x0 = 0; x0 < ow; x0 += tw) {
-      int x1 = std::min (x0 + tw, ow) - 1;
-      max_cols = std::max (max_cols, (int) (p->h.offset[x1] + p->h.span - p->h.offset[x0]));
-    }
+    const int max_rows = staged_extent (p->v, th, false).extent, max_cols = staged_extent (p->h, tw, false).extent;
     int pitch = (max_cols + 3) & ~3;
     int crows = p->cvshift ? max_rows / 2 + 3 : max_rows + 1;    // chroma rows staged per tile
     size_t planes = (size_t) 3 * max_rows * pitch;
@@ -383,16 +375,13 @@ bool fast_layout_ok (const VcsPlan * p)
 void std_pairs_check (VcsPlan * p)
 {
   bool std_pairs = !p->chroma_nearest && p->v_pairs && !p->in_422_444 && !p->rgb_in && !p->planes_mode &&
-      !(p->in.stride[0] & 7) && !(p->in.offset[0] & 7) && p->in.stride[0] >= ((p->in.width + 7) & ~7) && !(p->in.height & 1) &&
-      (int) p->chroma_mode.size () >= p->in.height;
+      !(p->in.stride[0] & 7) && !(p->in.offset[0] & 7) && p->in.stride[0] >= ((p->in.width + 7) & ~7) && !(p->in.height & 1);
   if (p->planar)                                  // I420 / YV12: 32-bit loads of 4 samples + the next one from each chroma plane
     for (int k = 1; k <= 2; k++)
       std_pairs = std_pairs && !(p->in.stride[k] & 3) && !(p->in.offset[k] & 3) && p->in.stride[k] >= ((((p->in.width + 7) & ~7) >> 1));
   else
     std_pairs = std_pairs && !(p->in.stride[1] & 7) && !(p->in.offset[1] & 7) && p->in.stride[1] >= ((p->in.width + 7) & ~7);
-  for (int y = 0; std_pairs && y < p->in.height; y++)
-    if (p->chroma_mode[y] != (y == 0 ? 0 : ((y & 1) ? 1 : 2))) std_pairs = false;
-  p->light_std_pairs = std_pairs;
+  p->light_std_pairs = std_pairs && standard_pairing (*p);
 }
 
 void light_geometry (VcsPlan * p)
@@ -404,53 +393,24 @@ void light_geometry (VcsPlan * p)
   // the packed 16-bit-lane lerps need fractions in [0,255] (h) and weights in [0,256] (v)
   if (p->h.mode == PASS_2TAP) for (int16_t c : p->h.coef) if (c < 0 || c > 255) return;
   if (p->v.mode == PASS_2TAP) for (int16_t c : p->v.coef) if (c < 0 || c > 256) return;
-  const int ow = p->out.width, oh = p->out.height, tw = 128;
+  const int tw = 128;
+  const StagedExtent x = staged_extent (p->h, tw, true);
+  if (!x.inside) return;
+  const int cp = x.extent + 4;                                    // +4 words: rows start on distinct banks
   const char *env_th = getenv ("B200_LIGHT_TH");              // tuning aid
   static const int heights[] = {32, 16, 8, 4, 2, 1};              // 32 rows first: fewest CTAs on C1
   for (int hi = 0; hi < 6; hi++) {
     const int th = (env_th && hi == 0) ? atoi (env_th) : heights[hi];
-    int max_rows = 0, max_cols = 0;
-    for (int y0 = 0; y0 < oh; y0 += th) {
-      int y1 = std::min (y0 + th, oh) - 1;
-      max_rows = std::max (max_rows, (int) (p->v.offset[y1] + p->v.span - p->v.offset[y0]));
-    }
-    for (int x0 = 0; x0 < ow; x0 += tw) {
-      int x1 = std::min (x0 + tw, ow) - 1;
-      int c0 = (int) p->h.offset[x0] & ~3, c1 = ((int) (p->h.offset[x1] + p->h.span) + 3) & ~3;
-      max_cols = std::max (max_cols, c1 - c0);
-    }
-    const int cp = max_cols + 4;                                  // +4 words: rows start on distinct banks
+    const StagedExtent y = staged_extent (p->v, th, false);
+    if (!y.inside) continue;
     const size_t t_words = p->h_first ? 0 : (size_t) th * cp;     // horizontal first: the two passes are fused, no intermediate tile
-    const size_t total = ((size_t) max_rows * cp + t_words + 4 * (size_t) max_rows + 4 + th) * 4;   // S, T, work list, v table
+    const size_t total = ((size_t) y.extent * cp + t_words + 4 * (size_t) y.extent + 4 + th) * 4;   // S, T, work list, v table
     if (total <= (env_th ? 200 : 96) * 1024) {
-      p->light_ok = true; p->light_tw = tw; p->light_th = th; p->light_rows = max_rows; p->light_cp = cp;
+      p->light_ok = true; p->light_tw = tw; p->light_th = th; p->light_rows = y.extent; p->light_cp = cp;
       p->light_smem = (int) total;
-
       return;
     }
   }
-}
-
-// 4 signed 8-bit taps per word, zero padded to a whole number of words; false when a tap does not
-// fit or the 16-bit accumulator of the reference could wrap (the kernel accumulates in 32 bits)
-bool pack_taps_s8 (const AxisPlan & a, int *ntw, std::vector<int32_t> * out)
-{
-  *ntw = 0; out->clear ();
-  if (a.mode != PASS_NTAP) return true;
-  const int n = a.n_taps, w = (n + 3) / 4;
-  out->assign ((size_t) a.out_size * w, 0);
-  for (int j = 0; j < a.out_size; j++) {
-    int mag = 0;
-    for (int k = 0; k < n; k++) {
-      const int t = a.coef[(size_t) j * n + k];
-      if (t < -128 || t > 127) return false;
-      mag += abs (t);
-      (*out)[(size_t) j * w + k / 4] |= (int32_t) ((uint32_t) (uint8_t) (int8_t) t << (8 * (k & 3)));
-    }
-    if (255 * mag + 32 > 32767) return false;
-  }
-  *ntw = w;
-  return true;
 }
 
 // Geometry of the n-tap kernel (vcs_ntap.cuh)
@@ -461,100 +421,29 @@ void ntap_geometry (VcsPlan * p)
   if (!(hn || vn) || p->h.mode == PASS_2TAP || p->v.mode == PASS_2TAP) return;
   if (!fast_layout_ok (p)) return;
   if (!pack_taps_s8 (p->h, &p->ntw_h, &p->h_packed) || !pack_taps_s8 (p->v, &p->ntw_v, &p->v_packed)) return;
-  p->ntap_alpha_opaque = true;
-  if (hn) for (int16_t s : p->h.sum) if (s < 64 || s > 128) p->ntap_alpha_opaque = false;
-  if (vn) for (int16_t s : p->v.sum) if (s < 64 || s > 128) p->ntap_alpha_opaque = false;
-  const int ow = p->out.width, oh = p->out.height;
-  // tile shape: the one that stages the fewest input pixels per output pixel (filter halos shrink
-  // with the tile) among those whose shared memory lets at least two CTAs share an SM
+  p->ntap_alpha_opaque = alpha_stays_opaque (p->h) && alpha_stays_opaque (p->v);
   static const int shapes[][2] = {{128, 32}, {128, 16}, {64, 32}, {128, 8}, {64, 16}, {32, 32}, {64, 8}, {32, 16},
                                   {64, 4}, {32, 8}, {32, 4}, {32, 2}, {32, 1}};
-  double best = 0;
-  const char *env_shape = getenv ("B200_NTAP_SHAPE");             // tuning aid: "tw,th"
-  int etw = 0, eth = 0;
-  if (env_shape && sscanf (env_shape, "%d,%d", &etw, &eth) != 2) etw = eth = 0;
-  for (auto & sh : shapes) {
-    const int tw = sh[0], th = sh[1];
-    if (etw && (tw != etw || th != eth)) continue;
-    if (th > 16 && oh < 2 * th) continue;
-    int max_rows = 0, max_cols = 0;
-    for (int y0 = 0; y0 < oh; y0 += th) {
-      int y1 = std::min (y0 + th, oh) - 1;
-      max_rows = std::max (max_rows, (int) (p->v.offset[y1] + p->v.span - p->v.offset[y0]));
-    }
-    for (int x0 = 0; x0 < ow; x0 += tw) {
-      int x1 = std::min (x0 + tw, ow) - 1;
-      int c0 = (int) p->h.offset[x0] & ~3, c1 = ((int) (p->h.offset[x1] + p->h.span) + 3) & ~3;
-      max_cols = std::max (max_cols, c1 - c0);
-    }
-    // rows: whole groups of 4; pitch (word columns per line): the zero-padded horizontal taps may
-    // read up to ntw_h + 1 words past the window start; the h-scaled tile keeps 1 + ntw_v groups of
-    // slack for the zero-padded vertical taps
-    const int rows = ((max_rows + 3) & ~3), ngr = rows / 4, groups = ngr + 1 + p->ntw_v;
-    const int pitch = max_cols / 4 + 2 + p->ntw_h;
-    const size_t s_words = ((size_t) ngr * 3 * pitch + 2) * 4;
-    const size_t t_words = (size_t) groups * tw * 4;
-    const size_t tap_words = (size_t) tw * std::max (p->ntw_h, 1) + (size_t) th * std::max (p->ntw_v, 1) + th;
-    size_t total = (s_words + t_words + tap_words + 4 * (size_t) rows + 12) * 4;
-    if (!p->h_first) {
+  auto smem = [p] (TileShape & t) -> size_t {
+    // rows: whole groups of 4; pitch (word columns per line): the zero-padded horizontal taps read words wi .. wi + ntw_h
+    // past the window start; the h-scaled tile keeps 1 + ntw_v groups of slack for the zero-padded vertical taps
+    const int ngr = t.rows / 4, groups = ngr + 1 + p->ntw_v;
+    t.pitch = t.cols / 4 + 2 + p->ntw_h;
+    if ((t.x.max_base >> 2) + p->ntw_h + 1 > t.pitch) return 0;
+    if (!p->h_first)
       // vertical first: plain planes S[3][rows][pitch], v-scaled rows T[3][th][pitch], 16-bit v taps one per word
-      total = ((size_t) 3 * rows * pitch + 4 + (size_t) 3 * th * pitch + 4 + (size_t) tw * std::max (p->ntw_h, 1) +
-          (size_t) th * std::max (p->v.n_taps, 1) + th + 4 * (size_t) rows + 12) * 4;
-    }
-    if (total > 100 * 1024) continue;
-    // staged input pixels + h-scaled pixels per output pixel; small tiles pay extra per-tile overhead
-    const double cost = ((double) rows * max_cols + (double) rows * tw) / ((double) std::min (tw, ow) * std::min (th, oh))
-        + 64.0 / th + 256.0 / tw;
-    if (!p->ntap_ok || cost < best) {
-      best = cost;
-      p->ntap_ok = true; p->ntap_tw = tw; p->ntap_th = th; p->ntap_rows = rows; p->ntap_pitch = pitch;
-      p->ntap_smem = (int) total;
-    }
-  }
-}
-
-// Walk every tile the fast kernels will run and check each shared-memory index range against the
-// geometry chosen above; a violation (none is known) downgrades the plan to the generic kernel instead
-// of risking an out-of-bounds access.  tests/test_host_plan.py sweeps random sizes over this.
-void validate_fast_geometry (VcsPlan * p)
-{
-  const int ow = p->out.width, oh = p->out.height;
-  auto tile_ok = [&] (int tw, int th, int rows_cap, int words_cap, int ntw_h, int extra_words) {
-    for (int y0 = 0; y0 < oh; y0 += th) {
-      const int y1 = std::min (y0 + th, oh) - 1;
-      const int R = (int) (p->v.offset[y1] + p->v.span - p->v.offset[y0]);
-      if (R > rows_cap || R < 1) return false;
-      for (int y = y0; y <= y1; y++) {                            // every output row's window inside the staged rows
-        const int rb = (int) p->v.offset[y] - (int) p->v.offset[y0];
-        if (rb < 0 || rb + p->v.span > R) return false;
-      }
-    }
-    for (int x0 = 0; x0 < ow; x0 += tw) {
-      const int x1 = std::min (x0 + tw, ow) - 1;
-      const int cxa = (int) p->h.offset[x0] & ~3, cx1 = (int) (p->h.offset[x1] + p->h.span);
-      const int ng = (cx1 - cxa + 3) >> 2;
-      if (ng + extra_words > words_cap) return false;
-      for (int x = x0; x <= x1; x++) {
-        const int base = (int) p->h.offset[x] - cxa;
-        if (base < 0 || base + p->h.span > cx1 - cxa) return false;
-        if ((base >> 2) + ntw_h + 1 > words_cap) return false;    // funnel-shift FIR reads words wi .. wi + ntw_h
-      }
-    }
-    return true;
+      return ((size_t) 3 * t.rows * t.pitch + 4 + (size_t) 3 * t.th * t.pitch + 4 + (size_t) t.tw * std::max (p->ntw_h, 1) +
+          (size_t) t.th * std::max (p->v.n_taps, 1) + t.th + 4 * (size_t) t.rows + 12) * 4;
+    if ((t.y.max_base >> 2) + p->ntw_v >= groups) return 0;      // vertical FIR over 4-line groups
+    const size_t s_words = ((size_t) ngr * 3 * t.pitch + 2) * 4;
+    const size_t t_words = (size_t) groups * t.tw * 4;
+    const size_t tap_words = (size_t) t.tw * std::max (p->ntw_h, 1) + (size_t) t.th * std::max (p->ntw_v, 1) + t.th;
+    return (s_words + t_words + tap_words + 4 * (size_t) t.rows + 12) * 4;
   };
-  if (p->light_ok && !tile_ok (p->light_tw, p->light_th, p->light_rows, p->light_cp / 4, 0, 0)) p->light_ok = false;
-  if (p->ntap_ok) {
-    bool ok = tile_ok (p->ntap_tw, p->ntap_th, p->ntap_rows, p->ntap_pitch, p->ntw_h, 0);
-    if (ok && p->h_first) {                                       // vertical FIR over 4-line groups: g0 + ntw_v < groups
-      const int groups = p->ntap_rows / 4 + 1 + p->ntw_v;
-      for (int y0 = 0; y0 < oh && ok; y0 += p->ntap_th)
-        for (int y = y0; y < std::min (y0 + p->ntap_th, oh); y++) {
-          const int rb = (int) p->v.offset[y] - (int) p->v.offset[y0];
-          if ((rb >> 2) + p->ntw_v >= groups) { ok = false; break; }
-        }
-    }
-    if (!ok) p->ntap_ok = false;
-  }
+  TileShape s;
+  if (!search_tile_shape (p->h, p->v, shapes, (int) std::size (shapes), "B200_NTAP_SHAPE", smem, &s)) return;
+  p->ntap_ok = true; p->ntap_tw = s.tw; p->ntap_th = s.th; p->ntap_rows = s.rows; p->ntap_pitch = s.pitch;
+  p->ntap_smem = (int) s.smem;
 }
 
 // setup_scale (video-converter.c:8092-8245) for planar in/out (4:2:0 same family; Y42B / Y444 -> I420 / YV12): what each output plane does
@@ -599,6 +488,92 @@ int build_planes (VcsPlan * p, const VideoFormatDesc & fi, const VideoFormatDesc
 }
 
 }  // namespace
+
+StagedExtent staged_extent (const AxisPlan & a, int tile, bool word_grid)
+{
+  StagedExtent e;
+  for (int i0 = 0; i0 < a.out_size; i0 += tile) {
+    const int i1 = std::min (i0 + tile, a.out_size) - 1;
+    const int start = (int) a.offset[i0] & (word_grid ? ~3 : ~0), end = (int) a.offset[i1] + a.span;
+    e.extent = std::max (e.extent, (word_grid ? (end + 3) & ~3 : end) - start);
+    for (int i = i0; i <= i1; i++) {
+      const int base = (int) a.offset[i] - start;
+      if (base < 0 || base + a.span > end - start) e.inside = false;
+      e.max_base = std::max (e.max_base, base);
+    }
+  }
+  return e;
+}
+
+bool search_tile_shape (const AxisPlan & h, const AxisPlan & v, const int (*shapes)[2], int n_shapes, const char *env,
+    const std::function<size_t (TileShape &)> & smem, TileShape * best)
+{
+  const int ow = h.out_size, oh = v.out_size;
+  const char *env_shape = getenv (env);
+  int etw = 0, eth = 0;
+  if (env_shape && sscanf (env_shape, "%d,%d", &etw, &eth) != 2) etw = eth = 0;
+  double best_cost = 0;
+  bool found = false;
+  for (int i = 0; i < n_shapes; i++) {
+    TileShape s;
+    s.tw = shapes[i][0]; s.th = shapes[i][1];
+    if (etw && (s.tw != etw || s.th != eth)) continue;
+    if (s.th > 16 && oh < 2 * s.th) continue;
+    s.x = staged_extent (h, s.tw, true); s.y = staged_extent (v, s.th, false);
+    if (!s.x.inside || !s.y.inside) continue;
+    s.rows = (s.y.extent + 3) & ~3; s.cols = s.x.extent;
+    s.smem = smem (s);
+    if (s.smem == 0 || s.smem > 100 * 1024) continue;
+    // staged input pixels + h-scaled pixels per output pixel; small tiles pay extra per-tile overhead
+    const double cost = ((double) s.rows * s.cols + (double) s.rows * s.tw) / ((double) std::min (s.tw, ow) * std::min (s.th, oh))
+        + 64.0 / s.th + 256.0 / s.tw;
+    if (!found || cost < best_cost) {
+      found = true; best_cost = cost; *best = s;
+    }
+  }
+  return found;
+}
+
+bool pack_taps_s8 (const AxisPlan & a, int *ntw, std::vector<int32_t> * out)
+{
+  *ntw = 0; out->clear ();
+  if (a.mode != PASS_NTAP) return true;
+  const int n = a.n_taps, w = (n + 3) / 4;
+  out->assign ((size_t) a.out_size * w, 0);
+  for (int j = 0; j < a.out_size; j++) {
+    int mag = 0;
+    for (int k = 0; k < n; k++) {
+      const int t = a.coef[(size_t) j * n + k];
+      if (t < -128 || t > 127) return false;
+      mag += abs (t);
+      (*out)[(size_t) j * w + k / 4] |= (int32_t) ((uint32_t) (uint8_t) (int8_t) t << (8 * (k & 3)));
+    }
+    if (255 * mag + 32 > 32767) return false;
+  }
+  *ntw = w;
+  return true;
+}
+
+int common_tap_words (int h_mode, int v_mode, int ntw_h, int ntw_v)
+{
+  if (h_mode == PASS_NTAP && v_mode == PASS_NTAP) return ntw_h == ntw_v ? ntw_h : 0;
+  return h_mode == PASS_NTAP ? ntw_h : ntw_v;
+}
+
+bool alpha_stays_opaque (const AxisPlan & a)
+{
+  if (a.mode == PASS_NTAP)
+    for (int16_t s : a.sum) if (s < 64 || s > 128) return false;
+  return true;
+}
+
+bool standard_pairing (const VcsPlan & p)
+{
+  if ((int) p.chroma_mode.size () < p.in.height) return false;
+  for (int y = 0; y < p.in.height; y++)
+    if (p.chroma_mode[y] != (y == 0 ? 0 : ((y & 1) ? 1 : 2))) return false;
+  return true;
+}
 
 // nibble k of the result: the input byte of the component that `out` stores at byte (or plane) k, for the components
 // `first` .. B (0 = A, 1 = R, 2 = G, 3 = B; pos[] of the format table)
@@ -981,7 +956,6 @@ static int build_chain_plan (VcsPlan * p, int pc, const VideoFormatDesc & fi, co
       std_pairs_check (p);
       light_geometry (p);
       ntap_geometry (p);
-      validate_fast_geometry (p);
     }
     return B200_OK;
   }
@@ -995,7 +969,6 @@ static int build_chain_plan (VcsPlan * p, int pc, const VideoFormatDesc & fi, co
   std_pairs_check (p);
   light_geometry (p);
   ntap_geometry (p);
-  validate_fast_geometry (p);
 
   // the specialised kernel covers exactly the headline shape class: even 2:1 in both
   // directions with the 8-tap lanczos the reference derives for it

@@ -6,7 +6,9 @@
 // line caches it produces flat tables the fused kernels index directly.
 #pragma once
 
+#include <stddef.h>
 #include <stdint.h>
+#include <functional>
 #include <vector>
 
 #include "../../include/b200dsp.h"
@@ -121,5 +123,40 @@ struct VcsPlan {
 // builds everything that does not need a device; returns b200_status
 int build_vcs_plan (const b200_video_info * in, const b200_video_info * out,
     const b200_vcs_config * cfg, VcsPlan * plan);
+
+// What the tiles of one axis stage, `tile` outputs to a tile: the input samples from the first output's window start
+// to the last output's window end; on the word grid from a 4-aligned start, the extent rounded up to whole words.
+struct StagedExtent {
+  int extent = 0;                // the most input samples any tile stages
+  int max_base = 0;              // the furthest an output's window starts from its tile's staged start
+  bool inside = true;            // every output's window [offset, offset + span) lies inside its tile's staged range
+};
+StagedExtent staged_extent (const AxisPlan & a, int tile, bool word_grid);
+
+// A tile shape of the dp4a kernels (n-tap, plane scaler): tw x th outputs, the staged lines rounded up to whole 4-line
+// groups, the staged columns on the word grid
+struct TileShape {
+  int tw = 0, th = 0, rows = 0, cols = 0;
+  StagedExtent x, y;
+  int pitch = 0;                 // words per staged line, set by the kernel's shared-memory formula
+  size_t smem = 0;
+};
+// The shape of `shapes` that stages the fewest input pixels per output pixel, among those whose windows lie inside
+// the staged ranges and whose shared memory lets at least two CTAs share an SM.  smem (shape) is the kernel's
+// formula: it sets shape.pitch and returns the bytes, 0 for a shape the kernel cannot run.  The environment variable
+// `env` ("tw,th", a tuning aid) restricts the search to that shape.  False when no shape qualifies.
+bool search_tile_shape (const AxisPlan & h, const AxisPlan & v, const int (*shapes)[2], int n_shapes, const char *env,
+    const std::function<size_t (TileShape &)> & smem, TileShape * best);
+
+// 4 signed 8-bit taps per word, zero padded to a whole number of words; false when a tap does not fit or the 16-bit
+// accumulator of the reference could wrap (the dp4a kernels accumulate in 32 bits).  ntw = 0 for other than n-tap axes.
+bool pack_taps_s8 (const AxisPlan & a, int *ntw, std::vector<int32_t> * out);
+// the tap-word count the dp4a kernels take as a template argument: the n-tap axis's, both axes' when they agree, else
+// 0 (counted at run time)
+int common_tap_words (int h_mode, int v_mode, int ntw_h, int ntw_v);
+// an n-tap axis whose every tap sum lies in [64, 128] keeps alpha at 255 (other axes do not touch it)
+bool alpha_stays_opaque (const AxisPlan & a);
+// every input line pulled in order with the standard 4:2:0 pairing: line 0 alone, then (1, 2), (3, 4) ...
+bool standard_pairing (const VcsPlan & p);
 
 }  // namespace b200

@@ -476,28 +476,6 @@ inline plane_fast_fn<ST> plane_fast_kernel_for (int hm, int vm, int nc, bool vfi
   return nullptr;
 }
 
-// 4 signed 8-bit taps per word, zero padded to whole words; false when a tap does not fit or the reference's 16-bit accumulator
-// could wrap (the kernel accumulates in 32 bits) - the rule of the n-tap kernel's tables (vcs_plan.cpp)
-inline bool plf_pack_taps_s8 (const AxisPlan & a, int *ntw, std::vector<int32_t> * out)
-{
-  *ntw = 0; out->clear ();
-  if (a.mode != PASS_NTAP) return true;
-  const int n = a.n_taps, w = (n + 3) / 4;
-  out->assign ((size_t) a.out_size * w, 0);
-  for (int j = 0; j < a.out_size; j++) {
-    int mag = 0;
-    for (int k = 0; k < n; k++) {
-      const int t = a.coef[(size_t) j * n + k];
-      if (t < -128 || t > 127) return false;
-      mag += abs (t);
-      (*out)[(size_t) j * w + k / 4] |= (int32_t) ((uint32_t) (uint8_t) (int8_t) t << (8 * (k & 3)));
-    }
-    if (255 * mag + 32 > 32767) return false;
-  }
-  *ntw = w;
-  return true;
-}
-
 // geometry + eligibility of one PM_SCALE plane; false leaves the plane to vcs_planes_kernel
 inline bool plan_plane_fast (const PlanePlan & q, int sstride, unsigned long long src_off, int dstride, unsigned long long dst_off,
     PlaneFastState * st, std::vector<int32_t> * hp, std::vector<int32_t> * vp)
@@ -510,65 +488,27 @@ inline bool plan_plane_fast (const PlanePlan & q, int sstride, unsigned long lon
   const AxisPlan & H = q.h, & V = q.v;
   if (H.mode < 1 || H.mode > 3 || V.mode < 1 || V.mode > 3) return false;
   int ntw_h = 0, ntw_v = 0;
-  if (!plf_pack_taps_s8 (H, &ntw_h, hp) || !plf_pack_taps_s8 (V, &ntw_v, vp)) return false;
+  if (!pack_taps_s8 (H, &ntw_h, hp) || !pack_taps_s8 (V, &ntw_v, vp)) return false;
   if (H.mode == PASS_2TAP) for (int16_t f : H.coef) if (f < 0 || f > 255) return false;     // 8-bit fractions (ldreslinb)
   if (V.mode == PASS_2TAP && !q.h_first) for (int16_t w : V.coef) if (w < 0 || w > 256) return false;   // lane form of lerp_v_u8
-  const int hspan = H.mode == PASS_NTAP ? H.n_taps : (H.mode == PASS_2TAP ? 2 : 1);
-  const int vspan = V.mode == PASS_NTAP ? V.n_taps : (V.mode == PASS_2TAP ? 2 : 1);
-  const int ow = q.ow, oh = q.oh;
   static const int shapes[][2] = {{128, 64}, {128, 32}, {128, 16}, {64, 32}, {128, 8}, {64, 16}, {32, 32}, {64, 8}, {32, 16},
                                   {64, 4}, {32, 8}, {32, 4}};
-  double best = 0; bool found = false;
-  const char *env_shape = getenv ("B200_PLF_SHAPE");               // tuning aid: "tw,th"
-  int etw = 0, eth = 0;
-  if (env_shape && sscanf (env_shape, "%d,%d", &etw, &eth) != 2) etw = eth = 0;
-  for (auto & sh : shapes) {
-    const int tw = sh[0], th = sh[1];
-    if (etw && (tw != etw || th != eth)) continue;
-    if (th > 16 && oh < 2 * th) continue;
-    int max_rows = 0, max_cols = 0;
-    bool ok = true;
-    for (int y0 = 0; y0 < oh && ok; y0 += th) {
-      const int y1 = std::min (y0 + th, oh) - 1;
-      const int R = (int) V.offset[y1] + vspan - (int) V.offset[y0];
-      if (R < 1) ok = false;
-      max_rows = std::max (max_rows, R);
-      for (int y = y0; y <= y1 && ok; y++) {                      // every row's window inside the staged lines, in order
-        const int rb = (int) V.offset[y] - (int) V.offset[y0];
-        if (rb < 0 || rb + vspan > R) ok = false;
-      }
-    }
-    for (int x0 = 0; x0 < ow && ok; x0 += tw) {
-      const int x1 = std::min (x0 + tw, ow) - 1;
-      const int c0 = (int) H.offset[x0] & ~3, c1 = (int) H.offset[x1] + hspan;
-      max_cols = std::max (max_cols, ((c1 + 3) & ~3) - c0);
-      for (int x = x0; x <= x1 && ok; x++) {
-        const int base = (int) H.offset[x] - c0;
-        if (base < 0 || base + hspan > c1 - c0) ok = false;
-      }
-    }
-    if (!ok) continue;
-    const int rows = (max_rows + 3) & ~3, ngr = rows / 4, groups = ngr + 1 + ntw_v;
-    const int pitch = max_cols / 4 + 2 + std::max (ntw_h, 1);
-    const size_t words = (q.h_first ? ((size_t) ngr * q.ne * pitch + 2) * 4 + (size_t) groups * tw * q.ne
-                                    : ((size_t) groups * q.ne * pitch + 2) * 4 + (size_t) th * q.ne * pitch) +
-        (size_t) tw * std::max (ntw_h, 1) + (size_t) th * std::max (ntw_v, 1) + th + 8;
-    const size_t total = words * 4;
-    if (total > 100 * 1024) continue;
-    const double cost = ((double) rows * max_cols + (double) rows * tw) / ((double) std::min (tw, ow) * std::min (th, oh))
-        + 64.0 / th + 256.0 / tw;
-    if (!found || cost < best) {
-      found = true; best = cost;
-      st->dev.tw = tw; st->dev.th = th; st->dev.rows = rows; st->dev.pitch = pitch; st->smem = total;
-    }
-  }
-  if (!found) return false;
+  auto smem = [&] (TileShape & t) -> size_t {
+    const int ngr = t.rows / 4, groups = ngr + 1 + ntw_v;
+    t.pitch = t.cols / 4 + 2 + std::max (ntw_h, 1);
+    return ((q.h_first ? ((size_t) ngr * q.ne * t.pitch + 2) * 4 + (size_t) groups * t.tw * q.ne
+                       : ((size_t) groups * q.ne * t.pitch + 2) * 4 + (size_t) t.th * q.ne * t.pitch) +
+        (size_t) t.tw * std::max (ntw_h, 1) + (size_t) t.th * std::max (ntw_v, 1) + t.th + 8) * 4;
+  };
+  TileShape s;
+  if (!search_tile_shape (H, V, shapes, (int) std::size (shapes), "B200_PLF_SHAPE", smem, &s)) return false;
   PlaneFastDev & d = st->dev;
+  d.tw = s.tw; d.th = s.th; d.rows = s.rows; d.pitch = s.pitch; st->smem = s.smem;
   d.src_off = src_off; d.dst_off = dst_off; d.sstride = sstride; d.dstride = dstride;
   d.iw = q.iw; d.ih = q.ih; d.ow = q.ow; d.oh = q.oh;
-  d.ntw_h = ntw_h; d.ntw_v = ntw_v; d.hspan = hspan; d.vspan = vspan; d.swz = q.swz;
+  d.ntw_h = ntw_h; d.ntw_v = ntw_v; d.hspan = H.span; d.vspan = V.span; d.swz = q.swz;
   st->hm = H.mode; st->vm = V.mode; st->nc = q.ne; st->vfirst = !q.h_first;
-  st->ntw = (H.mode == PASS_NTAP && V.mode == PASS_NTAP) ? (ntw_h == ntw_v ? ntw_h : 0) : (H.mode == PASS_NTAP ? ntw_h : ntw_v);
+  st->ntw = common_tap_words (H.mode, V.mode, ntw_h, ntw_v);
   st->ok = true;
   return true;
 }

@@ -153,10 +153,10 @@ def test_c5_filter_numbers_from_the_survey():
 
 
 def test_fast_kernel_selection_sweep():
-    """host-only plans over random sizes, methods and input formats: the plan builder validates every
-    shared-memory index range of the fast kernels tile by tile (validate_fast_geometry) and would fall back
-    to the generic kernel on a violation — for default layouts that must never happen for the common
-    methods at moderate ratios, and every plan must build"""
+    """host-only plans over random sizes, methods and input formats: the fast kernels' shape searches
+    (light_geometry, search_tile_shape) check every output's window against its tile's staged range and take
+    no shape that leaves it, which would fall back to the generic kernel — for default layouts that must
+    never happen for the common methods at moderate ratios, and every plan must build"""
     import gstreamer_b200 as g
     rng = np.random.default_rng(0)
     counts = {}
